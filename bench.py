@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """bench.py -- SSDNeRF hot-path benchmark (contract: see the task brief; numbers explained in DESIGN.md §6).
 
-    python bench.py --gpus N --steps K --warmup W            # this repo's sm_100a kernels
+    python bench.py --gpus N --steps K --warmup W            # this repo's sm_90a kernels
+    python bench.py ... --dump-outputs DIR                   # + what the last timed step computed, as DIR/<name>.npy
     python bench.py --impl reference --steps K --warmup W    # reference arithmetic on the host cores (oracle port)
 
 Workload (BASELINE.json configs[1]): `ssdnerf_cars_uncond`, batch 16 scenes per GPU, one STEP =
@@ -67,7 +68,8 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm_gbs=d['hbm_gbs'], tf_burst=d['bf16_tflops'], tf_sustained=d.get('bf16_tflops_sustained', d['bf16_tflops']), src='measured')
-    return dict(hbm_gbs=6650.0, tf_burst=1590.0, tf_sustained=1400.0, src='fallback')
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s -- what the hardware may reach, not a measurement
+    return dict(hbm_gbs=3350.0, tf_burst=989.0, tf_sustained=989.0, src='H100 SXM data sheet')
 
 
 class ClockSampler:
@@ -135,17 +137,32 @@ def build_model(dev, seed=0, rel='configs/paper_cfgs/ssdnerf_cars_uncond.py', te
     return model.to(dev).eval(), cfg
 
 
-def measured_traffic(kernel, rays):
-    """DRAM bytes per launch of `kernel` from a committed `ncu --set full` capture of this bench command (profiles/r02_render_traffic.json,
-    written by scripts/ncu_traffic.py from the .ncu-rep next to it); scaled by ray count when the capture used fewer views.  None when no
-    capture of the current kernel is committed -- never a hard-coded constant."""
-    path = os.path.join(ROOT, 'profiles', 'r02_render_traffic.json')
-    if not os.path.exists(path):
-        return None, None
-    d = json.load(open(path)).get(kernel)
-    if not d:
-        return None, None
-    return d['dram_bytes_per_launch'] * (rays / d['rays_per_launch']), f"profiles/r02_render_traffic.json ({d['source']})"
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, last, max_views=8, seed=0):
+    """The last timed step's outputs as float32 .npy files, at most DUMP_BYTES in all: the sampled triplanes `code` [B,3,C,H,W] and the
+    rendered `image` [B,V,h,w,3] / `depth` [B,V,h,w] (a full 251-view render is ~0.8 GB per batch of 16), restricted to a fixed seeded
+    choice of scenes (as many as fit half the budget) and of up to `max_views` views (as many as fit the rest); the chosen indices are
+    written alongside as `scene_indices` / `view_indices`."""
+    os.makedirs(out_dir, exist_ok=True)
+    code, image, depth = last['code'], last['image'], last['depth']
+    B, V = image.shape[0], image.shape[1]
+    rng = np.random.default_rng(seed)
+    code_per_scene = code[0].numel() * 4
+    n_scenes = max(1, min(B, (DUMP_BYTES // 2) // code_per_scene))
+    scenes = np.sort(rng.choice(B, size=n_scenes, replace=False))
+    view_bytes = n_scenes * (image[0, 0].numel() + depth[0, 0].numel()) * 4
+    n_views = max(0, min(max_views, V, (DUMP_BYTES - n_scenes * code_per_scene) // view_bytes))
+    views = np.sort(rng.choice(V, size=n_views, replace=False))
+    si = torch.as_tensor(scenes, device=code.device)
+    vi = torch.as_tensor(views, device=code.device, dtype=torch.long)
+    arrays = {'code': code.index_select(0, si), 'image': image.index_select(0, si).index_select(1, vi),
+              'depth': depth.index_select(0, si).index_select(1, vi)}
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, f'{name}.npy'), t.detach().float().cpu().numpy())
+    np.save(os.path.join(out_dir, 'scene_indices.npy'), scenes.astype(np.float64))
+    np.save(os.path.join(out_dir, 'view_indices.npy'), views.astype(np.float64))
 
 
 def run_ours(args):
@@ -207,6 +224,7 @@ def run_ours(args):
         e[3].record(stream)
         if rec is not None:
             rec.append(e)
+        last['code'], last['image'], last['depth'] = code, img, depth
         return img
 
     # ---- end-to-end through the plugin API with host buffers (+ the eval-side NCCL all-gather of 8-bit images when N > 1)
@@ -255,6 +273,7 @@ def run_ours(args):
         stream.wait_stream(copy_stream)                 # every device->host copy has landed before the closing event
 
     # ---- resident (kernel-side) measurement
+    last = {}
     for _ in range(args.warmup):
         resident_step()
     barrier()
@@ -269,6 +288,8 @@ def run_ours(args):
     barrier()
     clk = clocks.stop()
     total_ms = t0.elapsed_time(t1) / args.steps
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
     ddim_ms = float(np.mean([e[0].elapsed_time(e[1]) for e in rec]))
     dens_ms = float(np.mean([e[1].elapsed_time(e[2]) for e in rec]))
     rend_ms = float(np.mean([e[2].elapsed_time(e[3]) for e in rec]))
@@ -311,7 +332,7 @@ def run_ours(args):
         def render_s(counts=False):
             return R.render_fwd(R.DEC_S, planes_s, (128, 128), bits_s, dec_s.packed_blob(), poses=poses, intrinsics=intr, img_hw=(IMG, IMG),
                                 want_blend=True, want_counts=counts)
-        s_ms = timed(render_s, max(1, min(args.steps, 3)), 1)
+        s_ms = timed(render_s, args.steps, 1)
         s_samples = int(render_s(True)['num_samples'].sum().item())
         del code_s, planes_s
 
@@ -329,18 +350,18 @@ def run_ours(args):
         Sh.broadcast_scene(code1, bits1, 0)
         img, _ = model.render(decoder, code1, bits1, IMG, IMG, my_intr, my_poses, cfg=model.test_cfg)
         Sh.gather_views((img[0].clamp(0, 1) * 255.0 + 0.5).to(torch.uint8), V, out=ss_all, padded=ss_u8)
-    strong_ms = timed(strong_step, 10, 3)
+    strong_ms = timed(strong_step, args.steps, 3)
 
     # ---- stage-1 training step (every rank trains its own scenes; the shared decoder's gradient is all-reduced over NCCL inside the step)
     train = train2 = None
     if args.train:
-        train = train_measurement(dev, timed, rank)
-        train2 = train_stage2_measurement(dev, timed, rank)
+        train = train_measurement(dev, timed, rank, steps=args.steps)
+        train2 = train_stage2_measurement(dev, timed, rank, steps=args.steps)
 
     # ---- config-4 shape guided evaluations (rank 0): UNet forward + render loss forward/backward + UNet input-gradient pass
     guided = None
     if args.guided and rank == 0:
-        guided = guided_measurement(dev, ev, stream)
+        guided = guided_measurement(dev, ev, stream, evals=args.steps)
 
     # ---- reduce over ranks (max time)
     times = torch.tensor([total_ms, ddim_ms, dens_ms, rend_ms, e2e_ms, s_ms or 0.0, strong_ms, train['ms'] if train else 0.0,
@@ -363,7 +384,6 @@ def run_ours(args):
     tf_achieved = unet_flops / (ddim_ms * 1e-3) / 1e12
     render_bytes = (samples_all / world) * RAY_GATHER_BYTES_PER_SAMPLE + rays * RAY_IO_BYTES
     kern_p = os.environ.get('SSDNERF_BENCH_KERNEL_P', 'k_render_p3')
-    traffic, traffic_src = measured_traffic(kern_p, rays)
     gather_bytes = B * V * IMG * IMG * 3 * world if world > 1 else 0
     line = {
         'metric': METRIC, 'value': rays_per_s, 'unit': 'rays/s', 'triplanes_per_sec': trip_per_s,
@@ -373,7 +393,7 @@ def run_ours(args):
                                f'{IMG}x{IMG} render, batch {B}/GPU', 'global_batch': trip_all, 'rays_per_step': rays_all,
                    'samples_per_ray': samples_all / rays_all,
                    'parallelism': f'scenes x{world} (independent replicas; e2e adds the eval-side NCCL all-gather of 8-bit images)',
-                   'l2_policy': 'working set per step (activations > 1 GB, 66 M rays of output) exceeds the 126 MB L2; no flush needed'},
+                   'l2_policy': 'working set per step (activations > 1 GB, 66 M rays of output) exceeds the 50 MB L2 of an H100; no flush needed'},
         'stage_ms': {'ddim': ddim_ms, 'density': dens_ms, 'render': rend_ms},
         'e2e': {'value': rays_all / (e2e_ms * 1e-3), 'unit': 'rays/s', 'triplanes_per_sec': trip_all / (e2e_ms * 1e-3), 'ms_per_step': e2e_ms,
                 'path': 'DiffusionNeRF.val_step: H2D (noise, poses, intrinsics) + DDIM + density + render + D2H of the images (copy stream, overlaps the next DDIM)'
@@ -383,16 +403,14 @@ def run_ours(args):
         'gpu_launches': gpu_launches,
         'clocks': clk,
         # dominant kernel of the step = the fused renderer (~3/4 of the step): ALGORITHMIC gather + output bytes per launch / launch
-        # duration against the measured HBM copy peak (BASELINE.md 2c).  The planes (1.5 MB/scene) are L1/L2-resident, so real DRAM
-        # traffic (`traffic`, from the committed ncu capture) is far below the algorithmic bytes and the binding unit is the SM.
+        # duration against the HBM peak.  The planes (1.5 MB/scene) are L1/L2-resident, so real DRAM traffic is below the algorithmic bytes.
         'roofline': {'kernel': f'{kern_p} (fused march + gather + MLP + composite), one launch per step', 'bound': 'hbm',
                      'achieved': render_bytes / (rend_ms * 1e-3) / 1e9, 'peak': pk['hbm_gbs'], 'unit': 'GB/s',
-                     'frac': render_bytes / (rend_ms * 1e-3) / 1e9 / pk['hbm_gbs'], 'peak_source': pk['src'] + ' (burst copy)',
-                     'algorithmic_bytes_per_launch': render_bytes, 'samples_per_sec': samples_all / world / (rend_ms * 1e-3),
-                     'traffic': traffic, 'traffic_source': traffic_src},
-        'roofline_unet': {'kernel': 'k_gemm_tc / k_conv_row2 (tcgen05 implicit-GEMM conv / GEMM) + glue, timed as the whole DDIM stage', 'bound': 'tensor',
+                     'frac': render_bytes / (rend_ms * 1e-3) / 1e9 / pk['hbm_gbs'], 'peak_source': pk['src'],
+                     'algorithmic_bytes_per_launch': render_bytes, 'samples_per_sec': samples_all / world / (rend_ms * 1e-3)},
+        'roofline_unet': {'kernel': 'k_gemm_tc / k_conv_row2 (wgmma implicit-GEMM conv / GEMM) + glue, timed as the whole DDIM stage', 'bound': 'tensor',
                           'achieved': tf_achieved, 'peak': pk['tf_sustained'], 'unit': 'TFLOP/s', 'frac': tf_achieved / pk['tf_sustained'],
-                          'peak_source': f"{pk['src']} (sustained cuBLAS bf16)"},
+                          'peak_source': f"{pk['src']} (dense fp16 / bf16)"},
         'strong_scaling': {'workload': f'1 scene x {V} views x {IMG}x{IMG}, views sharded over {world} rank(s); per call: broadcast code + bitfield '
                                        f'from rank 0, render, all-gather 8-bit images' if world > 1 else f'1 scene x {V} views x {IMG}x{IMG} on one GPU',
                            'ms': strong_ms, 'rays_per_sec': V * IMG * IMG / (strong_ms * 1e-3), 'scaling': 'strong'},
@@ -600,7 +618,9 @@ def run_reference(args):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--gpus', type=int, default=1)
-    ap.add_argument('--steps', type=int, default=3)
+    ap.add_argument('--steps', type=int, default=3,
+                    help='timed iterations of every measured loop (resident, e2e, variant-S render, strong scaling, training steps) and '
+                         'the number of guided evaluations timed in one sampler call')
     ap.add_argument('--warmup', type=int, default=3)
     ap.add_argument('--impl', default='b200', choices=['b200', 'reference'])
     ap.add_argument('--batch', type=int, default=B_PER_GPU)
@@ -609,6 +629,8 @@ def main():
     ap.add_argument('--no-side-s', dest='side_s', action='store_false', help='skip the variant-S renderer workload')
     ap.add_argument('--no-guided', dest='guided', action='store_false', help='skip the config-4 guided-evaluation measurement')
     ap.add_argument('--no-train', dest='train', action='store_false', help='skip the stage-1 training-step measurement')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write the last step\'s triplanes and a fixed sample of its rendered views to DIR/<name>.npy')
     args = ap.parse_args()
     if args.warmup < 3 and args.impl == 'b200':
         args.warmup = 3      # timing rule: at least 3 warm-up steps

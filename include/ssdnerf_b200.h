@@ -1,5 +1,5 @@
 /*
- * ssdnerf_b200.h -- C ABI of libssdnerf_b200.so: B200 (sm_100a) kernels for SSDNeRF's two hot paths.
+ * ssdnerf_b200.h -- C ABI of libssdnerf_b200.so: H100 (sm_90a) kernels for SSDNeRF's two hot paths.
  *
  * Conventions (all entry points):
  *   - plain pointers + sizes, no torch / ATen types; every pointer is a DEVICE pointer owned by the
@@ -28,10 +28,10 @@ extern "C" {
 #define SSDNERF_OK 0
 #define SSDNERF_ERR_CUDA (-1)   /* a CUDA runtime / driver call failed */
 #define SSDNERF_ERR_ARG (-2)    /* invalid argument (shape, alignment, unsupported variant) */
-#define SSDNERF_ERR_ARCH (-3)   /* device is not sm_100 */
+#define SSDNERF_ERR_ARCH (-3)   /* device is not sm_90 */
 
 SSDNERF_API const char* ssdnerf_last_error(void);
-/* library version and the SM architecture it was compiled for (100) */
+/* library version and the SM architecture it was compiled for (90) */
 SSDNERF_API int ssdnerf_version(void);
 SSDNERF_API int ssdnerf_compiled_arch(void);
 /* number of CUDA kernels this library has launched (or recorded into a capturing stream) in this process */
@@ -96,13 +96,10 @@ SSDNERF_API int ssdnerf_sh_encode_backward(const float* grad, const float* input
 #define SSDNERF_DEC_P 0 /* shipped configs: base 3*6->64, density 64->1, dir_net 16->64, color 64->3
                            (configs/paper_cfgs/ssdnerf_cars_uncond.py:40-51) */
 #define SSDNERF_DEC_P_SIMT 2 /* decoder P on the CUDA cores in plain fp32 (csrc/render_fused.cu) */
-#define SSDNERF_DEC_P_TC 3   /* decoder P with the base layer as a split-precision fp16 tcgen05 GEMM (csrc/render_ptc.cu);
-                                SSDNERF_DEC_P selects the fastest P kernel (currently SSDNERF_DEC_P_MMA2, see DESIGN.md §3) */
 #define SSDNERF_DEC_P_MMA 4  /* decoder P, warp-synchronous: per-warp split-precision mma.sync base layer (csrc/render_p2.cu) */
 #define SSDNERF_DEC_P_MMA2 7 /* decoder P, warp-synchronous v2: one exponential per hidden unit shared by both branches, dir_net on the
                                 tensor cores, one reciprocal per four sigmoids (csrc/render_p3.cu); what SSDNERF_DEC_P selects */
-#define SSDNERF_DEC_S_TC 6   /* decoder S, CTA-synchronous tcgen05 kernel (csrc/render_tc.cu) */
-#define SSDNERF_DEC_S_MMA 5  /* decoder S, warp-synchronous mma.sync kernel (csrc/render_s2.cu); SSDNERF_DEC_S selects the faster one */
+#define SSDNERF_DEC_S_MMA 5  /* decoder S, warp-synchronous mma.sync kernel (csrc/render_s2.cu); what SSDNERF_DEC_S selects */
 #define SSDNERF_DEC_S 1 /* TriPlaneDecoder class defaults: base 3*32->128, density 128->1, color (128+16)->128->3
                            (lib/models/decoders/triplane_decoder.py:24-39) */
 
@@ -153,7 +150,7 @@ typedef struct ssdnerf_render_args {
     int32_t* num_samples;     /* samples composited per ray, optional */
     int32_t* voxel_trace;     /* optional [B][N][trace_cap] occupancy-bit index of every composited sample (-1 padded) */
     uint32_t trace_cap;
-    void* debug_phase_cycles; /* optional uint64[8]: per-phase clock64 totals of thread 0 of every CTA (SSDNERF_DEC_P_TC only) */
+    void* debug_phase_cycles; /* optional uint64[8]: per-phase clock64 totals of thread 0 of every CTA (SSDNERF_DEC_P / SSDNERF_DEC_P_MMA2: decode iterations, active lanes) */
     /* --- scratch */
     void* workspace;          /* >= ssdnerf_render_workspace_bytes(...) bytes, 16-byte aligned */
     size_t workspace_bytes;
@@ -234,7 +231,7 @@ SSDNERF_API int ssdnerf_density_pack(const void* density_grid, int grid_is_half,
                          void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * 4. UNet building blocks of the DDIM loop (tcgen05 tensor-core GEMM / implicit-GEMM convolution +
+ * 4. UNet building blocks of the DDIM loop (wgmma tensor-core GEMM / implicit-GEMM convolution +
  *    memory-bound glue kernels).  Activations are NHWC fp16; accumulation is fp32.
  *    replaces: cuDNN/cuBLAS calls under lib/models/architecture/ddpm/denoising.py:191-216 and
  *              modules.py:28-48 (+ mmgen 0.7.2 DenoisingResBlock / NormWithEmbedding / QKVAttention /
@@ -255,7 +252,7 @@ typedef struct ssdnerf_gemm_args {
      *    conv / plain: coordinate 2 = tap; b_batched: coordinates (2, 3) = the tile's (d2, d3) tile indices */
     const void* b; uint64_t b_strides[3]; uint32_t n, n_rows_b, bx2, bx3; uint32_t b_batched;
     uint32_t bn;              /* N tile: 0 = auto, else 64 / 128 / 256 */
-    uint32_t cluster;         /* 0 = auto, 1 = no cluster, 2 = CTA pairs along M with TMA multicast of the B tile */
+    uint32_t cluster;         /* 0 = auto (no cluster), 1 = no cluster, 2 / 4 / 8 = clusters along M with TMA multicast of the B tile */
     float alpha;
     const float* bias_n;      /* [n] fp32 or NULL */
     const void* residual;     /* fp16, addressed like out, or NULL */
@@ -263,7 +260,8 @@ typedef struct ssdnerf_gemm_args {
     /* optional fused GroupNorm statistics of the output: qstats [images][n/4][2] += {sum, sum of squares} of every 4-channel quad
      * (caller zero-fills); image of a row = index along d3 (stats_hw == 0) or (index along d1) / stats_hw (flattened rows) */
     float* qstats; uint32_t stats_hw;
-    void* debug_cycles;      /* optional uint64[8] device counters (pipeline wait cycles per role, summed over CTAs); NULL in production */
+    void* debug_cycles;      /* optional uint64[8] device counters of the generic tile kernel, clock cycles summed over CTAs: [0] producer wait
+                              * for a free stage, [1] producer total, [2] consumer wait for a full stage, [4] consumer total; NULL in production */
     uint32_t algo;           /* 0 = auto, 1 = generic tile kernel, 2 = row-pair 3x3 convolution (128-pixel rows, 128 output channels) */
     /* generalised K-slabs: taps in [1, 9] with tap_offsets[2t], [2t+1] = shift of slab t in (d1, d2) (NULL: the 3x3 / 1x1 defaults) --
      * e.g. the four 2x2-tap phase convolutions a nearest-x2 upsample + 3x3 convolution decomposes into;
@@ -312,7 +310,6 @@ typedef struct ssdnerf_conv_gn_args {
     void* out;                             /* [B][H][128][128] fp16 */
     float* qstats;                         /* optional [B][32][2] quad statistics of the output (caller zero-fills) */
     void* coef_workspace;                  /* device scratch, B * (C1 + C2) * 8 bytes, 16-byte aligned (per-image affine table) */
-    void* debug_cycles;                    /* optional uint64[8] pipeline wait counters (debug); NULL in production */
 } ssdnerf_conv_gn_args;
 SSDNERF_API int ssdnerf_conv3x3_gn_f16(const ssdnerf_conv_gn_args* args, void* stream);
 /* fused attention: out[b][t][h*ch + d] = softmax_s(scale * q[b,t,h,:] . k[b,s,h,:]) v[b,s,h,d], scores kept on chip (flash-style);

@@ -1,4 +1,4 @@
-"""Builds libssdnerf_b200.so in-tree with nvcc for sm_100a (no JIT cache: the .so travels with the repo).
+"""Builds libssdnerf_b200.so in-tree with nvcc for sm_90a (no JIT cache: the .so travels with the repo).
 
 Every csrc/*.cu is compiled to an object under ssdnerf_b200/_obj/ (git-ignored) in parallel and only when it or a header changed,
 then linked; `python -m ssdnerf_b200.build [--force] [-v]`."""
@@ -15,7 +15,7 @@ LIB = os.path.join(HERE, 'libssdnerf_b200.so')
 
 NVCC_FLAGS = [
     '-O3', '-std=c++17', '-lineinfo',
-    '-gencode', 'arch=compute_100a,code=sm_100a',
+    '-gencode', 'arch=compute_90a,code=sm_90a',
     '-Xcompiler', '-fPIC,-fvisibility=hidden',
     '--expt-relaxed-constexpr',
 ]

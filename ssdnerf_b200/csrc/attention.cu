@@ -7,7 +7,7 @@
 // K / V tiles double-buffered in shared memory with cp.async.  q, k, v are read in place from the qkv projection output with the
 // reference's legacy head layout (head h owns channels [3 ch h, 3 ch (h + 1)) = q | k | v).
 // Work is tiny next to the convolutions (17 GFLOP per block at 32x32): the point is removing 0.5 GB of score traffic per block,
-// not tensor-pipe utilisation, so the legacy warp-level MMA is the right tool (no TMEM round trip per 64-key tile).
+// not tensor-pipe utilisation, so the legacy warp-level MMA is the right tool (no shared-memory round trip of the scores per 64-key tile).
 #include "common.cuh"
 #include "../../include/ssdnerf_b200.h"
 #include <cuda_fp16.h>
@@ -182,7 +182,7 @@ extern "C" int ssdnerf_flash_attn(const void* qkv, uint32_t B, uint32_t T, uint3
     // 128 queries per CTA (8 warps) when the sequence is long enough to still fill the GPU, else 64 (SSDNERF_FA_WARPS=4|8 overrides)
     static int force = -1;
     if (force < 0) { const char* e = getenv("SSDNERF_FA_WARPS"); force = e ? atoi(e) : 0; }
-    const bool wide = force == 8 && T % 128 == 0;      // measured on B200 (T = 1024, ch = 64, 64 heads): 8 warps 86 us, 4 warps 75 us -> 4 is the default
+    const bool wide = force == 8 && T % 128 == 0;      // 4 warps (64 queries per CTA) is the default
     if (ch == 64) return wide ? launch_flash<64, 8>((const __half*)qkv, B, T, heads, scale, (__half*)out, (cudaStream_t)stream)
                               : launch_flash<64, 4>((const __half*)qkv, B, T, heads, scale, (__half*)out, (cudaStream_t)stream);
     if (ch == 128) return wide ? launch_flash<128, 8>((const __half*)qkv, B, T, heads, scale, (__half*)out, (cudaStream_t)stream)

@@ -1,4 +1,4 @@
-// Shared device helpers for the ssdnerf_b200 CUDA kernels (sm_100a only).
+// Shared device helpers for the ssdnerf_b200 CUDA kernels (sm_90a).
 //
 // The occupancy-grid stepping arithmetic is pinned with explicit intrinsics so the
 // integer outputs (voxel / morton / bit indices, per-ray sample counts) are bit-exact
@@ -40,9 +40,16 @@ struct DeviceOnce {
     bool done[64] = {};
     bool first() { const int d = current_device(); if (done[d]) return false; done[d] = true; return true; }
 };
+// multiprocessor count of the current device (queried once per device): grid sizing of the element-wise kernels
+inline uint32_t device_sms() {
+    static int sms[64] = {};
+    const int d = current_device();
+    if (!sms[d]) { int n = 0; (void)cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, d); sms[d] = n > 0 ? n : 1; }
+    return (uint32_t)sms[d];
+}
 
 // Programmatic dependent launch (PDL): consecutive kernels of the DDIM step are launched with the programmatic-stream-serialization
-// attribute, so the next kernel's CTAs may start (barrier init, TMEM allocation, weight / bias staging) while the tail of the current
+// attribute, so the next kernel's CTAs may start (barrier init, weight / bias staging) while the tail of the current
 // one drains.  pdl_wait() blocks until the preceding kernel has completed and its writes are visible: nothing produced by an earlier
 // kernel may be read, and nothing an earlier kernel reads may be written, before it.  Both are no-ops for ordinary launches.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }

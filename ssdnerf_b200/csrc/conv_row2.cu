@@ -1,230 +1,337 @@
-// 3x3 convolution, 128-pixel-wide images, 128 output channels (the UNet's 128 x 128 level): row-pair kernel with horizontal halo reuse.
+// 3x3 convolution for the UNet's 128 x 128 level (128-pixel rows, 128 output channels): row-pair kernel with horizontal and vertical
+// halo reuse, optionally fused with the GroupNorm(32) [+ NormWithEmbedding scale / shift] + SiLU that precedes the convolution.
 //
-// The generic implicit-GEMM kernel (gemm_tc.cu) stages, per 64-channel k-block and per tap, a 128 x 64 activation tile and a
-// 128 x 64 weight tile for ONE 128 x 128 x 64 product: 32 KB of shared memory traffic per 2.1 MFLOP, and its operand pipeline
-// (shared-memory stages x bytes per stage / load round trip) saturates at ~58 B/clk/SM -- half of what the tensor pipe could eat
-// at N = 128 (profiles/r01_gemm_pipeline_*.txt).  This kernel makes every staged byte do 2.4x more work:
-//   * a tile is TWO image rows (y0, y0+1) of one image -> two TMEM accumulators share every weight tile;
-//   * per (ky, 64-channel chunk) ONE activation box of 2 rows x 130 pixels (x = -1 .. 128, zero-filled out of bounds by TMA) serves
-//     the three horizontal taps: tap kx reads rows [kx, kx + 128) of the box through a shifted shared-memory descriptor
-//     (K-major SWIZZLE_128B, start address advanced by kx rows of 128 B; the matrix-base-offset field stays 0 -- measured: the
-//     128B swizzle phase of a row is taken from its absolute shared-memory address, exactly as TMA wrote it).
-// Staged bytes per (ky, chunk): 33 KB activations + 3 x 16 KB weights for 6 products of 128 x 128 x 64 (13.5 KB per product).
-// Roles as in gemm_tc.cu: warp 0 TMA producer, warp 1 MMA issuer (converged warp, elected lane), warps 2..9 epilogue
-// (bias, residual, fp16 store, fused GroupNorm quad statistics).
+// Replaces on the reference path (mmgen DenoisingResBlock.forward as used by lib/models/architecture/ddpm/modules.py:51-110):
+//     conv3x3(x)  and  conv3x3( SiLU( GroupNorm(x) * (1 + scale) + shift ) )  -- the latter without materialising the normalised input.
+//
+// A tile is TWO output rows (y0, y0 + 1) of one image.  Per 64-channel chunk, the loader warpgroup reads the 4 input rows y0-1 .. y0+2
+// (130 pixels each, x = -1 .. 128, zero outside the image) ONCE, applies the GroupNorm affine a x + b in fp32 and SiLU as h + h tanh(h),
+// h = u / 2, on packed halves (tanh.approx.f16x2) when fused, and stores them in the K-major SWIZZLE_128B row layout (16-byte chunk index
+// XOR (pixel & 7)).  Zero padding is written as literal zeros (it pads the activation, not the raw input).  Consumer warpgroup a
+// accumulates output row y0 + a (2 x 64 pixels x 128 channels, fp32 in registers): for tap (ky, kx) it reads its A fragments from input
+// row ky + a shifted by kx pixels with ldmatrix and issues register-A wgmma against the tap's 128 x 64 weight tile (TMA, SWIZZLE_128B).
+// Every staged input row serves up to 6 taps, every weight tile both output rows.
 #include "common.cuh"
 #include "tc_common.cuh"
 #include "conv_row_epilogue.cuh"
 #include "../../include/ssdnerf_b200.h"
 #include <cuda_fp16.h>
-#include <cstdlib>
 
 namespace ssdnerf {
 using namespace tc;
 
-constexpr int kRwThreads = 320, kRwEpi = 256;
-constexpr int kRwABox = 2 * 130 * 128;                  // bytes of one activation box: 2 rows x 130 pixels x 64 halves
-constexpr int kRwASlot = 33 * 1024;                     // slot stride (1024-aligned)
-constexpr int kRwBSlot = kRwN * 128;                    // 16 KB weight tile
-constexpr int kRwAStages = 2, kRwBStages = 7;          // pair mode: 3 activation slots, 8 half-size weight stages
-constexpr size_t kRwSmemTail = 1024 /*align*/ + 256 /*barriers*/ + 512 /*qacc*/ + 512 /*bias*/ + 8 * 2048 /*epilogue staging*/;
-constexpr size_t kRwSmem = (size_t)kRwAStages * kRwASlot + (size_t)kRwBStages * kRwBSlot + kRwSmemTail;           // single CTA
-constexpr size_t kRwSmemPair = (size_t)3 * kRwASlot + (size_t)8 * (kRwBSlot / 2) + kRwSmemTail;                    // per CTA of a pair
+constexpr int kRwThreads = 384;                          // warpgroups 0, 1: consumers (output rows y0, y0 + 1); warpgroup 2: row loaders
+constexpr int kRwRowSlot = 17 * 1024;                    // one staged input row: 130 pixels x 64 halves = 16.25 KB, 1024-aligned slots
+constexpr int kRwBSlot = kRwN * 128;                     // 16 KB weight tile (128 output channels x 64 input channels)
+constexpr int kRwRows = 6, kRwBStages = 6;
+constexpr int kGnMaxC = 384;
+constexpr size_t kRwSmem = (size_t)kRwRows * kRwRowSlot + (size_t)kRwBStages * kRwBSlot + 1024 /*align*/ + 256 /*barriers*/ +
+                           256 /*qacc*/ + 512 /*bias*/;
 
 struct ConvRowParams {
-    uint32_t B, H;                // images, rows (H even)
-    uint32_t kc1, kc2;            // 64-channel chunks from input 1 / input 2 (skip concat)
-    const float* bias;            // [128] or NULL
-    const __half* residual;       // NHWC [B][H][128][128] or NULL
-    __half* out;                  // NHWC [B][H][128][128]
-    float* qstats;                // optional [B][32][2]
-    unsigned long long* prof;
+    uint32_t B, H;                              // images, rows (H even)
+    const __half* x1; uint32_t C1;              // input [B][H][128][C1] addressed with element strides xs1 {pixel, row, image}
+    const __half* x2; uint32_t C2;              // optional second input (skip concat along channels)
+    long long xs1[3], xs2[3];
+    const float2* coef;                         // fused GroupNorm: [B][C1 + C2] per-(image, channel) affine {a, b} from k_gn_coef; NULL: plain
+    const float* bias;                          // [128] or NULL
+    const __half* residual;                     // NHWC [B][H][128][128] or NULL
+    __half* out;                                // NHWC [B][H][128][128]
+    float* qstats;                              // optional [B][32][2]
 };
 
-// PAIR: two CTAs (a cluster of 2 = the SMs of one TPC) work on two consecutive tiles with ONE tcgen05.mma.cta_group::2 of M = 256 per
-// (tap, accumulator): the leader's MMA reads each CTA's own 128 activation rows and half of the weight tile from each CTA, so the number
-// of issued MMA instructions -- what paces the single-CTA kernel at ~100 cycles per instruction against 64 cycles of execution
-// (profiles/r01_gemm_pipeline_prof.txt) -- and the staged weight bytes per SM both halve.
-template <bool PAIR>
+template <bool GN>
 __global__ void __launch_bounds__(kRwThreads, 1)
-k_conv_row2(const __grid_constant__ CUtensorMap mapA1, const __grid_constant__ CUtensorMap mapA2, const __grid_constant__ CUtensorMap mapB,
-            const ConvRowParams p) {
+k_conv_row2(const __grid_constant__ CUtensorMap mapB, const ConvRowParams p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    constexpr int kAStages = PAIR ? 3 : kRwAStages, kBStages = PAIR ? 8 : kRwBStages, kBSlot = PAIR ? kRwBSlot / 2 : kRwBSlot;
-    uint8_t* sA = smem;
-    uint8_t* sB = smem + kAStages * kRwASlot;
-    uint64_t* fullA = reinterpret_cast<uint64_t*>(sB + kBStages * kBSlot);
-    uint64_t* emptyA = fullA + kAStages;
-    uint64_t* fullB = emptyA + kAStages;
-    uint64_t* emptyB = fullB + kBStages;
-    uint64_t* tfull = emptyB + kBStages;
-    uint64_t* tempty = tfull + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
-    float* qacc = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(fullA) + 256);      // [32 quads][2]
-    float* sbias = qacc + 128;                                                             // [128]
-    uint8_t* sstage = reinterpret_cast<uint8_t*>(sbias + 128);                              // [8 warps][32 rows][64 B]
+    uint8_t* sR = smem;                                               // input row ring
+    uint8_t* sB = smem + kRwRows * kRwRowSlot;                        // weight stages
+    uint64_t* fullR = reinterpret_cast<uint64_t*>(sB + kRwBStages * kRwBSlot);
+    uint64_t* emptyR = fullR + kRwRows;
+    uint64_t* fullB = emptyR + kRwRows;
+    uint64_t* emptyB = fullB + kRwBStages;
+    float* qacc = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(fullR) + 256);       // [32 quads][2]
+    float* sbias = qacc + 64;                                                               // [128]
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
     const uint32_t tiles_per_img = p.H / 2, total_tiles = p.B * tiles_per_img;
-    const uint32_t KC = p.kc1 + p.kc2;
-    const uint32_t crank = PAIR ? cluster_ctarank() : 0u;
-    // this CTA's tiles: single CTA: blockIdx.x, + gridDim.x, ...; pair: cluster c owns tiles 2c + rank, stride 2 x #clusters
-    const uint32_t tile0 = PAIR ? cluster_id_x() * 2u + crank : blockIdx.x;
-    const uint32_t tstep = PAIR ? num_clusters_x() * 2u : gridDim.x;
+    const uint32_t kc1 = p.C1 / 64, KC = (p.C1 + p.C2) / 64;
+    const uint32_t tile0 = blockIdx.x, tstep = gridDim.x;
+    const uint32_t my_tiles = tile0 < total_tiles ? (total_tiles - tile0 + tstep - 1) / tstep : 0;
 
-    if (warp == 0 && lane == 0) {
-        prefetch_tmap(&mapA1); prefetch_tmap(&mapA2); prefetch_tmap(&mapB);
-        for (int i = 0; i < kAStages; ++i) { mbar_init(&fullA[i], 1); mbar_init(&emptyA[i], 1); }
-        for (int i = 0; i < kBStages; ++i) { mbar_init(&fullB[i], 1); mbar_init(&emptyB[i], 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&tfull[i], 1); mbar_init(&tempty[i], kRwEpi * (PAIR ? 2 : 1)); }   // pair: both epilogues free the leader's
+    if (threadIdx.x == 0) {
+        prefetch_tmap(&mapB);
+        // a staged row is released by all 8 consumer warps (each once it holds the last fragments it needs), filled by the 4 loader warps
+        for (int i = 0; i < kRwRows; ++i) { mbar_init(&fullR[i], 4); mbar_init(&emptyR[i], 8); }
+        for (int i = 0; i < kRwBStages; ++i) { mbar_init(&fullB[i], 1); mbar_init(&emptyB[i], 8); }
         fence_mbar_init();
     }
-    if (warp == 1) { if (PAIR) tmem_alloc2(tmem_slot, 512); else tmem_alloc(tmem_slot, 512); }
     for (int i = threadIdx.x; i < 64; i += kRwThreads) qacc[i] = 0.0f;
     for (int i = threadIdx.x; i < kRwN; i += kRwThreads) sbias[i] = p.bias ? __ldg(p.bias + i) : 0.0f;
-    tc_fence_before();
     __syncthreads();
-    if (PAIR) cluster_sync_all();        // the peer's barriers exist before any remote arrive / TMA completion targets them
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     pdl_trigger();
     pdl_wait();
 
-    if (warp == 0) {   // ---------------- TMA producer (pair: own activation box + own half of the weight tile, bytes credited to the leader)
-        uint32_t sa = 0, pa = 0, sb = 0, pb = 0;
+    // register budget: setmaxnreg moves registers within the CTA's launch-time pool (384 x 168): 128 x 120 + 256 x 192 = 384 x 168 (no spills in either role)
+    if (wg == 2) {   // ---------------- row loaders: raw rows -> (GroupNorm affine + SiLU) -> swizzled operand rows
+        setmaxnreg_dec<120>();
+        const uint32_t lt = threadIdx.x - 256u;                       // 0..127
+        const uint32_t c8 = lt & 7u, p0 = lt >> 3;                    // 16-byte chunk (8 channels) of the 64-channel row; pixels p0 + 16 n
+        const uint32_t C = p.C1 + p.C2;
+        uint32_t idx = 0;                                             // ring position of the row being produced
         for (uint32_t tile = tile0; tile < total_tiles; tile += tstep) {
             const uint32_t b = tile / tiles_per_img, y0 = (tile - b * tiles_per_img) * 2;
-            for (uint32_t ky = 0; ky < 3; ++ky) {
-                for (uint32_t j = 0; j < KC; ++j) {
-                    mbar_wait(&emptyA[sa], pa ^ 1);
-                    const bool first = j < p.kc1;
-                    const int ak = (int)((first ? j : j - p.kc1) * 64);
-                    if (!PAIR) {
-                        mbar_expect_tx_w(&fullA[sa], kRwABox);
-                        tma_load_4d_w(sA + sa * kRwASlot, first ? &mapA1 : &mapA2, &fullA[sa], ak, -1, (int)(y0 + ky) - 1, (int)b);
-                    } else {
-                        if (crank == 0) mbar_expect_tx_w(&fullA[sa], 2 * kRwABox);
-                        tma_load_4d_2cta_w(sA + sa * kRwASlot, first ? &mapA1 : &mapA2, mapa_u32(smem_u32(&fullA[sa]), 0), ak, -1, (int)(y0 + ky) - 1, (int)b);
-                    }
-                    if (++sa == kAStages) { sa = 0; pa ^= 1; }
-                    for (uint32_t kx = 0; kx < 3; ++kx) {
-                        mbar_wait(&emptyB[sb], pb ^ 1);
-                        if (!PAIR) {
-                            mbar_expect_tx_w(&fullB[sb], kRwBSlot);
-                            tma_load_4d_w(sB + sb * kBSlot, &mapB, &fullB[sb], (int)(j * 64), 0, (int)(ky * 3 + kx), 0);
-                        } else {
-                            if (crank == 0) mbar_expect_tx_w(&fullB[sb], kRwBSlot);
-                            tma_load_4d_2cta_w(sB + sb * kBSlot, &mapB, mapa_u32(smem_u32(&fullB[sb]), 0), (int)(j * 64), (int)(crank * 64), (int)(ky * 3 + kx), 0);
-                        }
-                        if (++sb == kBStages) { sb = 0; pb ^= 1; }
+            for (uint32_t j = 0; j < KC; ++j) {
+                const bool first = j < kc1;
+                const __half* src = first ? p.x1 : p.x2;
+                const long long xs0 = first ? p.xs1[0] : p.xs2[0], xs1 = first ? p.xs1[1] : p.xs2[1], xs2 = first ? p.xs1[2] : p.xs2[2];
+                const uint32_t cl = (first ? j : j - kc1) * 64u + c8 * 8u;
+                float ca[8], cb[8];
+                if (GN) {   // {a, b} of this thread's 8 channels, halved: SiLU(u) = h + h tanh(h) with h = u / 2
+                    const float4* cp = reinterpret_cast<const float4*>(p.coef + (size_t)b * C + j * 64u + c8 * 8u);
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) {
+                        const float4 t = __ldg(cp + k);
+                        ca[2 * k] = 0.5f * t.x; cb[2 * k] = 0.5f * t.y; ca[2 * k + 1] = 0.5f * t.z; cb[2 * k + 1] = 0.5f * t.w;
                     }
                 }
-            }
-        }
-        __syncwarp();
-    } else if (warp == 1) {   // ---------------- MMA issuer (pair: the leader issues for both SMs)
-      if (!PAIR || crank == 0) {
-        constexpr uint32_t idesc = make_idesc_f16(PAIR ? 256 : 128, kRwN);
-        constexpr uint16_t kBoth = 3;
-        uint32_t sa = 0, pa = 0, sb = 0, pb = 0, acc = 0, acc_phase = 0;
-        long long wf = 0; const long long mt0 = clock64();
-        for (uint32_t tile = tile0; tile < total_tiles; tile += tstep) {
-            if (PAIR) mbar_wait_cluster(&tempty[acc], acc_phase ^ 1); else mbar_wait(&tempty[acc], acc_phase ^ 1);
-            tc_fence_after();
-            const uint32_t d_tmem = tmem_base + acc * 256;
-            uint32_t started = 0;
-            for (uint32_t ky = 0; ky < 3; ++ky) {
-                for (uint32_t j = 0; j < KC; ++j) {
-                    if (p.prof) { const long long c = clock64(); mbar_wait(&fullA[sa], pa); wf += clock64() - c; } else mbar_wait(&fullA[sa], pa);
-                    const uint32_t a_base = smem_u32(sA + sa * kRwASlot);
-                    for (uint32_t kx = 0; kx < 3; ++kx) {
-                        if (p.prof) { const long long c = clock64(); mbar_wait(&fullB[sb], pb); wf += clock64() - c; } else mbar_wait(&fullB[sb], pb);
-                        tc_fence_after();
-                        const uint64_t b_desc = make_desc_sw128(smem_u32(sB + sb * kBSlot));
+                for (uint32_t r = 0; r < 4; ++r) {
+                    const int y = (int)(y0 + r) - 1;
+                    const bool row_ok = y >= 0 && y < (int)p.H;
+                    const __half* rowp = src + (long long)b * xs2 + (long long)(row_ok ? y : 0) * xs1 + cl;
+                    uint4 v[9];
 #pragma unroll
-                        for (uint32_t a = 0; a < 2; ++a) {
-                            const uint32_t row0 = a * 130 + kx;
-                            const uint64_t a_desc = make_desc_sw128(a_base + row0 * 128);
+                    for (int n = 0; n < 9; ++n) {
+                        const int x = (int)(p0 + 16u * n) - 1;
+                        v[n] = (row_ok && (unsigned)x < (unsigned)kRwW) ? __ldg(reinterpret_cast<const uint4*>(rowp + (long long)x * xs0))
+                                                                       : make_uint4(0, 0, 0, 0);
+                    }
+                    const uint32_t slot = idx % kRwRows;
+                    mbar_wait(&emptyR[slot], ((idx / kRwRows) & 1u) ^ 1u);
+                    const uint32_t dst = smem_u32(sR + slot * kRwRowSlot);
 #pragma unroll
-                            for (uint32_t k = 0; k < 4; ++k) {
-                                if (PAIR) umma_f16_2cta_w(d_tmem + a * kRwN, a_desc + 2 * k, b_desc + 2 * k, idesc, (started | k) != 0);
-                                else umma_f16_w(d_tmem + a * kRwN, a_desc + 2 * k, b_desc + 2 * k, idesc, (started | k) != 0);
+                    for (int n = 0; n < 9; ++n) {
+                        const uint32_t px = p0 + 16u * n;
+                        if (px >= 130u) continue;
+                        uint4 o = v[n];
+                        if (GN) {
+                            const bool ok = row_ok && (unsigned)((int)px - 1) < (unsigned)kRwW;
+                            const __half2* h = reinterpret_cast<const __half2*>(&v[n]);
+                            uint32_t* ow = reinterpret_cast<uint32_t*>(&o);
+#pragma unroll
+                            for (int k = 0; k < 4; ++k) {
+                                const float2 tt = __half22float2(h[k]);
+                                const __half2 hh = __floats2half2_rn(fmaf(tt.x, ca[2 * k], cb[2 * k]), fmaf(tt.y, ca[2 * k + 1], cb[2 * k + 1]));
+                                uint32_t hv = *reinterpret_cast<const uint32_t*>(&hh), tv;
+                                asm("tanh.approx.f16x2 %0, %1;" : "=r"(tv) : "r"(hv));
+                                const __half2 yy = __hfma2(hh, *reinterpret_cast<const __half2*>(&tv), hh);
+                                ow[k] = ok ? *reinterpret_cast<const uint32_t*>(&yy) : 0u;
                             }
                         }
-                        started = 1;
-                        if (PAIR) umma_commit_2cta_w(&emptyB[sb], kBoth); else umma_commit_w(&emptyB[sb]);
-                        if (++sb == kBStages) { sb = 0; pb ^= 1; }
+                        sts128(dst + px * 128u + ((c8 ^ (px & 7u)) << 4), o);
                     }
-                    if (PAIR) umma_commit_2cta_w(&emptyA[sa], kBoth); else umma_commit_w(&emptyA[sa]);
-                    if (++sa == kAStages) { sa = 0; pa ^= 1; }
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&fullR[slot]);
+                    ++idx;
                 }
             }
-            if (PAIR) umma_commit_2cta_w(&tfull[acc], kBoth); else umma_commit_w(&tfull[acc]);
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
         }
-        if (p.prof && lane == 0) { atomicAdd(p.prof + 2, (unsigned long long)wf); atomicAdd(p.prof + 4, (unsigned long long)(clock64() - mt0)); }
-      }
-        __syncwarp();
-    } else {   // ---------------- epilogue warps 2..9 (conv_row_epilogue.cuh)
-        const RowEpiArgs ea{p.H, p.residual, p.out, p.qstats};
-        conv_row_epilogue<8, PAIR>(ea, warp, lane, total_tiles, tiles_per_img, tmem_base, tfull, tempty, sstage, sbias, qacc, tile0, tstep);
+    } else {   // ---------------- consumers: warpgroup a accumulates output row y0 + a
+        setmaxnreg_inc<192>();
+        const uint32_t a = (uint32_t)wg, wq = (uint32_t)warp & 3u, cq = (uint32_t)lane & 3u;
+        const uint32_t steps_per_tile = KC * 9u, total_steps = my_tiles * steps_per_tile;
+        // weight tiles are issued by thread 0 in (tile, chunk, tap) order, kRwBStages ahead of the consumers
+        auto issue_w = [&](uint32_t L) {
+            const uint32_t s = L % kRwBStages;
+            if (L >= (uint32_t)kRwBStages) mbar_wait(&emptyB[s], ((L / kRwBStages) - 1u) & 1u);
+            mbar_expect_tx(&fullB[s], (uint32_t)kRwBSlot);
+            const uint32_t rem = L % steps_per_tile;
+            tma_load_4d(sB + s * kRwBSlot, &mapB, &fullB[s], (int)((rem / 9u) * 64u), 0, (int)(rem % 9u), 0);
+        };
+        if (threadIdx.x == 0)
+            for (uint32_t L = 0; L < total_steps && L < (uint32_t)kRwBStages; ++L) issue_w(L);
+        auto release_row = [&](uint32_t ring) { if (lane == 0) mbar_arrive(&emptyR[ring % kRwRows]); };
+        uint32_t m = 0, ridx = 0;
+        const uint32_t lrow = wq * 16u + ((uint32_t)lane & 15u);      // ldmatrix: pixel (within a 64-pixel half) whose row this lane addresses
+        const uint32_t lk = (uint32_t)lane >> 4;                      // ldmatrix: 8-channel half of the 16-channel k step
+        for (uint32_t tile = tile0; tile < total_tiles; tile += tstep) {
+            const uint32_t b = tile / tiles_per_img, y0 = (tile - b * tiles_per_img) * 2;
+            float acc0[64], acc1[64];                                 // pixels 0..63 / 64..127 of the row
+#pragma unroll
+            for (int i = 0; i < 64; ++i) { acc0[i] = 0.0f; acc1[i] = 0.0f; }
+            for (uint32_t j = 0; j < KC; ++j) {
+                // the input row this output row never reads (row 3 for a = 0, row 0 for a = 1) is released once it has been filled: an
+                // arrival before that could complete the phase of the slot's previous occupant while the other warpgroup still reads it
+                const uint32_t unused = ridx + (a == 0 ? 3u : 0u);
+                if (a == 1) { mbar_wait(&fullR[unused % kRwRows], (unused / kRwRows) & 1u); release_row(unused); }
+                for (uint32_t ky = 0; ky < 3; ++ky) {
+                    const uint32_t ring = ridx + ky + a;
+                    mbar_wait(&fullR[ring % kRwRows], (ring / kRwRows) & 1u);
+                    const uint32_t rowS = smem_u32(sR + (ring % kRwRows) * kRwRowSlot);
+                    for (uint32_t kx = 0; kx < 3; ++kx) {
+                        const uint32_t sb = m % kRwBStages;
+                        uint32_t af[2][4][4];
+#pragma unroll
+                        for (uint32_t h = 0; h < 2; ++h) {
+                            const uint32_t px = 64u * h + lrow + kx;        // staged pixel 0 is x = -1
+#pragma unroll
+                            for (uint32_t k = 0; k < 4; ++k) ldmatrix_x4(rowS + px * 128u + (((2u * k + lk) ^ (px & 7u)) << 4), af[h][k]);
+                        }
+                        if (kx == 2) release_row(ring);
+                        mbar_wait(&fullB[sb], (m / kRwBStages) & 1u);
+                        const uint64_t b_desc = make_desc_sw128(smem_u32(sB + sb * kRwBSlot));
+                        wgmma_fence();
+                        fence_regs(acc0); fence_regs(acc1);
+#pragma unroll
+                        for (uint32_t k = 0; k < 4; ++k) {
+                            wgmma_rs_n128(acc0, af[0][k], b_desc + 2 * k, 1u);
+                            wgmma_rs_n128(acc1, af[1][k], b_desc + 2 * k, 1u);
+                        }
+                        wgmma_commit();
+                        wgmma_wait<0>();
+                        fence_regs(acc0); fence_regs(acc1);
+                        if (lane == 0) mbar_arrive(&emptyB[sb]);
+                        if (threadIdx.x == 0 && m >= 1 && m - 1 + kRwBStages < total_steps) issue_w(m - 1 + kRwBStages);
+                        ++m;
+                    }
+                }
+                if (a == 0) { mbar_wait(&fullR[unused % kRwRows], (unused / kRwRows) & 1u); release_row(unused); }
+                ridx += 4;
+            }
+            // ---------------- epilogue: bias, residual, fp16 store, fused GroupNorm quad statistics of the fp32 values
+            const size_t pix0 = ((size_t)b * p.H + y0 + a) * kRwW;
+#pragma unroll
+            for (int i = 0; i < 16; ++i) {
+                const uint32_t ch = 8u * i + 2u * cq;
+                const float b0 = sbias[ch], b1 = sbias[ch + 1];
+                float su = 0.0f, sq = 0.0f;
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+#pragma unroll
+                    for (int hh = 0; hh < 2; ++hh) {
+                        const size_t o = (pix0 + 64u * h + wq * 16u + ((uint32_t)lane >> 2) + 8u * hh) * kRwN + ch;
+                        float v0 = (h ? acc1 : acc0)[4 * i + 2 * hh] + b0, v1 = (h ? acc1 : acc0)[4 * i + 2 * hh + 1] + b1;
+                        if (p.residual) { const float2 r = __half22float2(*reinterpret_cast<const __half2*>(p.residual + o)); v0 += r.x; v1 += r.y; }
+                        *reinterpret_cast<__half2*>(p.out + o) = __floats2half2_rn(v0, v1);
+                        su += v0 + v1; sq = fmaf(v0, v0, fmaf(v1, v1, sq));
+                    }
+                }
+                if (p.qstats) {
+                    frag_quad_reduce(su, sq);
+                    if ((lane & ~2) == 0) { float* qa = qacc + (2 * i + (lane >> 1)) * 2; atomicAdd(qa, su); atomicAdd(qa + 1, sq); }
+                }
+            }
+            if (p.qstats) {
+                asm volatile("bar.sync 1, 256;" ::: "memory");
+                if (threadIdx.x < 64) {
+                    const float val = qacc[threadIdx.x];
+                    if (val != 0.0f) atomicAdd(p.qstats + (size_t)b * 64 + threadIdx.x, val);
+                    qacc[threadIdx.x] = 0.0f;
+                }
+                asm volatile("bar.sync 1, 256;" ::: "memory");
+            }
+        }
     }
-    tc_fence_before();
     __syncthreads();
-    if (PAIR) cluster_sync_all();        // nobody exits while the leader's MMAs may still read its shared memory
-    if (warp == 1) { tc_fence_after(); if (PAIR) tmem_dealloc2(tmem_base, 512); else tmem_dealloc(tmem_base, 512); }
+}
+
+// per-(image, channel) GroupNorm affine, k_gn_apply arithmetic: y = x * a + b,
+//   a = rstd * gamma * (1 + scale), b = (beta - mean * rstd * gamma) * (1 + scale) + shift;  grid = images, one thread per channel (looped)
+__global__ void k_gn_coef(const float* __restrict__ q1, uint32_t C1, const float* __restrict__ q2, uint32_t C2, uint32_t HW,
+                          const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ scale_shift,
+                          long long ss_batch_stride, float eps, float2* __restrict__ coef) {
+    pdl_trigger();
+    pdl_wait();
+    __shared__ float2 s_mr[32];
+    const uint32_t b = blockIdx.x, C = C1 + C2, cpg = C / 32u;
+    const float inv_n = 1.0f / ((float)HW * (float)cpg);
+    if (threadIdx.x < 32u) {
+        const uint32_t q1n = C1 / 4, q2n = C2 / 4, nq = cpg / 4;
+        float sm = 0.0f, sq = 0.0f;
+        for (uint32_t i = 0; i < nq; ++i) {
+            const uint32_t qi = threadIdx.x * nq + i;
+            const float2 t = __ldg(reinterpret_cast<const float2*>(qi < q1n ? q1 + ((size_t)b * q1n + qi) * 2 : q2 + ((size_t)b * q2n + (qi - q1n)) * 2));
+            sm += t.x; sq += t.y;
+        }
+        const float mean = sm * inv_n;
+        s_mr[threadIdx.x] = make_float2(mean, rsqrtf(fmaxf(sq * inv_n - mean * mean, 0.0f) + eps));
+    }
+    __syncthreads();
+    const float* ss = scale_shift ? scale_shift + (size_t)b * ss_batch_stride : nullptr;
+    for (uint32_t c = threadIdx.x; c < C; c += blockDim.x) {
+        const float2 mr = s_mr[c / cpg];
+        const float ak = mr.y * __ldg(gamma + c);
+        const float bk = __ldg(beta + c) - mr.x * ak;
+        const float sc = ss ? 1.0f + __ldg(ss + c) : 1.0f, sh = ss ? __ldg(ss + C + c) : 0.0f;
+        coef[(size_t)b * C + c] = make_float2(ak * sc, fmaf(bk, sc, sh));
+    }
 }
 
 // tensor-map helper shared with gemm_tc.cu
 int make_map_4d_box(CUtensorMap* m, const void* base, uint64_t K, uint64_t e1, uint64_t e2, uint64_t e3, uint64_t s1, uint64_t s2, uint64_t s3,
                     uint32_t x1, uint32_t x2, uint32_t x3);
 
-// a: validated by ssdnerf_gemm_f16 (taps == 9, d1 == 128, b1 == 128, n == 128, fp16 output, dense NHWC output strides)
-int conv_row2_launch(const ssdnerf_gemm_args* a, int sms, cudaStream_t stream) {
-    ConvRowParams p{};
-    p.B = a->d3; p.H = a->d2; p.kc1 = a->k1 / 64; p.kc2 = a->a2 ? a->k2 / 64 : 0;
-    p.bias = a->bias_n; p.residual = (const __half*)a->residual; p.out = (__half*)a->out; p.qstats = a->qstats;
-    p.prof = (unsigned long long*)a->debug_cycles;
-    const uint64_t ktot = (uint64_t)a->k1 + (a->a2 ? a->k2 : 0);
-    CUtensorMap mA1, mA2, mB;
-    if (int e = make_map_4d_box(&mA1, a->a1, a->k1, a->d1, a->d2, a->d3, a->a1_strides[0], a->a1_strides[1], a->a1_strides[2], 130, 2, 1)) return e;
-    if (a->a2) {
-        if (int e = make_map_4d_box(&mA2, a->a2, a->k2, a->d1, a->d2, a->d3, a->a2_strides[0], a->a2_strides[1], a->a2_strides[2], 130, 2, 1)) return e;
-    } else {
-        mA2 = mA1;
+template <bool GN>
+static int launch_row2(const CUtensorMap& mB, const ConvRowParams& p, int sms, cudaStream_t stream) {
+    static DeviceOnce attr;
+    if (attr.first()) {
+        SSDNERF_CUDA_OK(cudaFuncSetAttribute(k_conv_row2<GN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRwSmem));
     }
     const uint32_t total = p.B * (p.H / 2);
-    // CTA pairs need an even tile count per image (pairs never straddle images); SSDNERF_ROW2_PAIR=0 forces the single-CTA kernel
-    static int pair_env = -1;
-    if (pair_env < 0) { const char* e = getenv("SSDNERF_ROW2_PAIR"); pair_env = e ? atoi(e) : 1; }
-    const bool pair = pair_env && (p.H / 2) % 2 == 0 && total >= 2;
-    if (int e = make_map_4d_box(&mB, a->b, ktot, a->n_rows_b ? a->n_rows_b : a->n, a->bx2 ? a->bx2 : 1, a->bx3 ? a->bx3 : 1, a->b_strides[0],
-                                a->b_strides[1], a->b_strides[2], pair ? kRwN / 2 : kRwN, 1, 1)) return e;
-    if (pair) {
-        static DeviceOnce attr;
-        if (attr.first()) {
-            SSDNERF_CUDA_OK(cudaFuncSetAttribute(k_conv_row2<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRwSmemPair));
-        }
-        const uint32_t clusters = (total / 2 < (uint32_t)sms / 2) ? total / 2 : (uint32_t)sms / 2;
-        cudaLaunchConfig_t cfg{};
-        cfg.gridDim = dim3(clusters * 2); cfg.blockDim = dim3(kRwThreads); cfg.dynamicSmemBytes = kRwSmemPair; cfg.stream = stream;
-        cudaLaunchAttribute at[2];
-        at[0].id = cudaLaunchAttributeClusterDimension;
-        at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-        at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        at[1].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-        cfg.attrs = at; cfg.numAttrs = 2;
-        SSDNERF_CUDA_OK(cudaLaunchKernelEx(&cfg, k_conv_row2<true>, mA1, mA2, mB, p));
-    } else {
-        static DeviceOnce attr;
-        if (attr.first()) {
-            SSDNERF_CUDA_OK(cudaFuncSetAttribute(k_conv_row2<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRwSmem));
-        }
-        SSDNERF_CUDA_OK(launch_pdl(k_conv_row2<false>, dim3(total < (uint32_t)sms ? total : (uint32_t)sms), dim3(kRwThreads), kRwSmem, stream, mA1, mA2, mB, p));
-    }
+    SSDNERF_CUDA_OK(launch_pdl(k_conv_row2<GN>, dim3(total < (uint32_t)sms ? total : (uint32_t)sms), dim3(kRwThreads), kRwSmem, stream, mB, p));
     SSDNERF_LAUNCH_OK();
     return 0;
 }
 
+// a: validated by ssdnerf_gemm_f16 (taps == 9, d1 == 128, b1 == 128, n == 128, fp16 output, dense NHWC output strides)
+int conv_row2_launch(const ssdnerf_gemm_args* a, int sms, cudaStream_t stream) {
+    if (((uintptr_t)a->a1 & 15u) || ((a->a1_strides[0] | a->a1_strides[1] | a->a1_strides[2]) & 15u) ||
+        (a->a2 && (((uintptr_t)a->a2 & 15u) || ((a->a2_strides[0] | a->a2_strides[1] | a->a2_strides[2]) & 15u))) ||
+        ((uintptr_t)a->out & 3u) || ((uintptr_t)a->residual & 3u))
+        return set_error_msg(SSDNERF_ERR_ARG, "gemm: row-pair convolution needs 16-byte aligned inputs and strides, 4-byte aligned output / residual");
+    ConvRowParams p{};
+    p.B = a->d3; p.H = a->d2;
+    p.x1 = (const __half*)a->a1; p.C1 = a->k1;
+    p.x2 = (const __half*)a->a2; p.C2 = a->a2 ? a->k2 : 0;
+    for (int i = 0; i < 3; ++i) { p.xs1[i] = (long long)(a->a1_strides[i] / 2); p.xs2[i] = a->a2 ? (long long)(a->a2_strides[i] / 2) : 0; }
+    p.bias = a->bias_n; p.residual = (const __half*)a->residual; p.out = (__half*)a->out; p.qstats = a->qstats;
+    const uint64_t ktot = (uint64_t)a->k1 + (a->a2 ? a->k2 : 0);
+    CUtensorMap mB;
+    if (int e = make_map_4d_box(&mB, a->b, ktot, a->n_rows_b ? a->n_rows_b : a->n, a->bx2 ? a->bx2 : 1, a->bx3 ? a->bx3 : 1, a->b_strides[0],
+                                a->b_strides[1], a->b_strides[2], kRwN, 1, 1)) return e;
+    return launch_row2<false>(mB, p, sms, stream);
+}
+
 }  // namespace ssdnerf
+
+using namespace ssdnerf;
+
+extern "C" int ssdnerf_conv3x3_gn_f16(const ssdnerf_conv_gn_args* a, void* stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    if (!a || !a->x1 || !a->q1 || !a->gamma || !a->beta || !a->w || !a->out || !a->coef_workspace)
+        return set_error_msg(SSDNERF_ERR_ARG, "conv3x3_gn: x1, q1, gamma, beta, w, out and coef_workspace are required");
+    if (a->B == 0 || a->H == 0) return 0;
+    if (a->H % 2) return set_error_msg(SSDNERF_ERR_ARG, "conv3x3_gn: H must be even (tiles are row pairs)");
+    if (a->C1 == 0 || a->C1 % 64 || a->C2 % 64 || (a->x2 && !a->q2)) return set_error_msg(SSDNERF_ERR_ARG, "conv3x3_gn: channel counts must be multiples of 64; x2 needs q2");
+    const uint32_t C = a->C1 + (a->x2 ? a->C2 : 0);
+    if (C > (uint32_t)kGnMaxC || (C / 32) % 4) return set_error_msg(SSDNERF_ERR_ARG, "conv3x3_gn: at most 384 input channels, channels per group a multiple of 4");
+    if (a->w_rows < 128) return set_error_msg(SSDNERF_ERR_ARG, "conv3x3_gn: packed weight needs >= 128 rows per tap");
+    if (((uintptr_t)a->x1 | (uintptr_t)a->x2 | (uintptr_t)a->out | (uintptr_t)a->residual | (uintptr_t)a->w | (uintptr_t)a->coef_workspace) & 15u)
+        return set_error_msg(SSDNERF_ERR_ARG, "conv3x3_gn: tensors must be 16-byte aligned");
+    ConvRowParams p{};
+    p.B = a->B; p.H = a->H; p.x1 = (const __half*)a->x1; p.C1 = a->C1; p.x2 = (const __half*)a->x2; p.C2 = a->x2 ? a->C2 : 0;
+    p.xs1[0] = p.C1; p.xs1[1] = (long long)kRwW * p.C1; p.xs1[2] = (long long)p.H * kRwW * p.C1;
+    p.xs2[0] = p.C2; p.xs2[1] = (long long)kRwW * p.C2; p.xs2[2] = (long long)p.H * kRwW * p.C2;
+    p.coef = (const float2*)a->coef_workspace; p.bias = a->bias; p.residual = (const __half*)a->residual; p.out = (__half*)a->out; p.qstats = a->qstats;
+    int dev = 0, sms = 0;
+    SSDNERF_CUDA_OK(cudaGetDevice(&dev));
+    SSDNERF_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    SSDNERF_CUDA_OK(launch_pdl(k_gn_coef, dim3(a->B), dim3(128), 0, stream, a->q1, a->C1, a->x2 ? a->q2 : (const float*)nullptr, p.C2, a->H * 128u,
+                               a->gamma, a->beta, a->scale_shift, a->ss_batch_stride, a->eps, (float2*)a->coef_workspace));
+    SSDNERF_LAUNCH_OK();
+    CUtensorMap mB;
+    if (int e = make_map_4d_box(&mB, a->w, C, a->w_rows, 9, 1, (uint64_t)C * 2, (uint64_t)a->w_rows * C * 2, (uint64_t)9 * a->w_rows * C * 2,
+                                kRwN, 1, 1)) return e;
+    return launch_row2<true>(mB, p, sms, stream);
+}

@@ -1,153 +1,18 @@
-// Epilogue shared by the row-pair convolution kernels (conv_row2.cu, conv_row2_gn.cu): warps 2..9, TMEM lane quarter = warp % 4
-// (pixels of a row), column half = (warp - 2) / 4; per tile two accumulators (image rows y0, y0 + 1) of 128 pixels x 128 channels at
-// TMEM columns acc * 256 + a * 128.  bias (shared memory) + residual + fp16 store through per-warp staging tiles (8 pixels x 64 contiguous
-// bytes per warp instruction) + fused GroupNorm quad statistics of the fp32 values.
+// Pieces shared by the wgmma GEMM (gemm_tc.cu) and the row-pair convolution (conv_row2.cu): the fused GroupNorm quad-statistics
+// reduction over a warp's accumulator fragment.
 #pragma once
 #include "common.cuh"
-#include "tc_common.cuh"
-#include <cuda_fp16.h>
 
 namespace ssdnerf {
 
-constexpr int kRwW = 128, kRwN = 128;                   // image width (pixels per row) and output channels
+constexpr int kRwW = 128, kRwN = 128;                   // row-pair convolution: image width (pixels per row) and output channels
 
-struct RowEpiArgs {
-    uint32_t H;
-    const __half* residual;       // NHWC [B][H][128][128] or NULL
-    __half* out;                  // NHWC [B][H][128][128]
-    float* qstats;                // optional [B][32][2]
-};
-
-// NW = 8: warps 2..9, column half = (warp - 2) / 4;  NW = 4: warps 2..5, each warp walks both column halves
-// PAIR: the kernel runs as a CTA pair (one tcgen05.mma.cta_group::2 per two CTAs): tiles are indexed by cluster, `tile0` / `tstep`
-// are this CTA's first tile and stride, and the accumulator-free signal goes to the LEADER CTA's barrier
-template <int NW, bool PAIR = false>
-__device__ __forceinline__ void conv_row_epilogue(const RowEpiArgs& p, int warp, int lane, uint32_t total_tiles, uint32_t tiles_per_img,
-                                                  uint32_t tmem_base, uint64_t* tfull, uint64_t* tempty, uint8_t* sstage,
-                                                  const float* sbias, float* qacc, uint32_t tile0 = blockIdx.x, uint32_t tstep = gridDim.x) {
-    using namespace tc;
-    const uint32_t q = (uint32_t)warp & 3u, hsel = (NW == 8) ? (uint32_t)(warp - 2) >> 2 : 0u;
-    constexpr int kIts = (NW == 8) ? 4 : 8;               // (row a, column half, 32-column chunk) steps per warp and tile
-    const uint32_t x = q * 32 + (uint32_t)lane;
-    uint32_t acc = 0, acc_phase = 0;
-    for (uint32_t tile = tile0; tile < total_tiles; tile += tstep) {
-        const uint32_t b = tile / tiles_per_img, y0 = (tile - b * tiles_per_img) * 2;
-        // global accesses re-mapped through a per-warp staging tile: one warp instruction = 8 pixels x 64 contiguous bytes (see gemm_tc.cu)
-        const uint32_t wst = smem_u32(sstage) + (uint32_t)(warp - 2) * 2048u;     // shared-space address of this warp's staging tile
-        const uint32_t pc = (uint32_t)lane & 3u;
-        uint32_t st_own[4], st_map[4];     // swizzled byte offsets: own row (lane) piece g / re-mapped row (lane >> 2) + 8 i piece pc
+// {sum, sum of squares} of one 8-column block of a wgmma accumulator fragment (each thread holds two rows x two columns of it,
+// masked by the caller) -> quad totals over the warp's 16 rows: lane 0 ends with quad 0 (columns 0..3), lane 2 with quad 1 (4..7)
+__device__ __forceinline__ void frag_quad_reduce(float& su, float& sq) {
+    su += __shfl_xor_sync(0xffffffffu, su, 1); sq += __shfl_xor_sync(0xffffffffu, sq, 1);
 #pragma unroll
-        for (int g = 0; g < 4; ++g) {
-            st_own[g] = wst + (uint32_t)lane * 64u + (((uint32_t)g ^ (((uint32_t)lane >> 1) & 3u)) << 4);
-            const uint32_t r = ((uint32_t)lane >> 2) + 8u * g;
-            st_map[g] = wst + r * 64u + ((pc ^ ((r >> 1) & 3u)) << 4);
-        }
-        const size_t offq = (((size_t)b * p.H + y0) * kRwW + q * 32) * kRwN + hsel * 64;      // pixel q*32 of row y0, this warp's first column half
-        // step it -> row a, column offset (relative to hsel * 64) cr: NW = 8: a = it >> 1, cr = 32 (it & 1); NW = 4: a = it >> 2, cr = 32 (it & 3)
-        auto step_a = [](int it) { return (uint32_t)(NW == 8 ? it >> 1 : it >> 2); };
-        auto step_c = [](int it) { return (uint32_t)(NW == 8 ? (it & 1) * 32 : (it & 3) * 32); };
-        uint4 rcur[4], rnext[4];
-        auto fetch_res = [&](size_t off, uint4* r) {      // off: element offset of pixel q*32 for the wanted (row, chunk)
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-                r[i] = p.residual ? __ldg(reinterpret_cast<const uint4*>(p.residual + off + (size_t)(((uint32_t)lane >> 2) + 8u * i) * kRwN + pc * 8))
-                                  : make_uint4(0, 0, 0, 0);
-        };
-        fetch_res(offq, rcur);
-        mbar_wait(&tfull[acc], acc_phase);
-        tc_fence_after();
-#pragma unroll
-        for (int it = 0; it < kIts; ++it) {
-            const uint32_t a = step_a(it);
-            const uint32_t c0 = hsel * 64 + step_c(it);
-            const size_t off = offq + (size_t)a * kRwW * kRwN + step_c(it);
-            uint32_t v[32];
-            tmem_ld32(tmem_base + ((q * 32u) << 16) + acc * 256 + a * kRwN + c0, v);
-            if (it + 1 < kIts) fetch_res(offq + (size_t)step_a(it + 1) * kRwW * kRwN + step_c(it + 1), rnext);
-            uint4 rrow[4];
-            if (p.residual) {
-#pragma unroll
-                for (int i = 0; i < 4; ++i) sts128(st_map[i], rcur[i]);
-                __syncwarp();
-#pragma unroll
-                for (int g = 0; g < 4; ++g) rrow[g] = lds128(st_own[g]);
-                __syncwarp();
-            }
-            tmem_ld_wait();
-            float f[32];
-#pragma unroll
-            for (int g = 0; g < 8; ++g) {
-                const float4 bv = *reinterpret_cast<const float4*>(sbias + c0 + 4 * g);
-                f[4 * g] = __uint_as_float(v[4 * g]) + bv.x; f[4 * g + 1] = __uint_as_float(v[4 * g + 1]) + bv.y;
-                f[4 * g + 2] = __uint_as_float(v[4 * g + 2]) + bv.z; f[4 * g + 3] = __uint_as_float(v[4 * g + 3]) + bv.w;
-            }
-            if (p.residual) {
-#pragma unroll
-                for (int g = 0; g < 4; ++g) {
-                    const __half2* h2 = reinterpret_cast<const __half2*>(&rrow[g]);
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) { const float2 t = __half22float2(h2[i]); f[8 * g + 2 * i] += t.x; f[8 * g + 2 * i + 1] += t.y; }
-                }
-            }
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-                uint4 o;
-                __half2* h2 = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-                for (int i = 0; i < 4; ++i) h2[i] = __floats2half2_rn(f[8 * g + 2 * i], f[8 * g + 2 * i + 1]);
-                sts128(st_own[g], o);
-            }
-            __syncwarp();
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const uint32_t r = ((uint32_t)lane >> 2) + 8u * i;
-                *reinterpret_cast<uint4*>(p.out + off + (size_t)r * kRwN + pc * 8) = lds128(st_map[i]);
-            }
-            __syncwarp();
-            if (p.qstats) {   // fused GroupNorm quad statistics (same reduce-scatter as gemm_tc.cu)
-                float sv[16];
-#pragma unroll
-                for (int q4 = 0; q4 < 8; ++q4) {
-                    float su = 0.0f, sq = 0.0f;
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) { const float xv = f[4 * q4 + e]; su += xv; sq = fmaf(xv, xv, sq); }
-                    sv[q4] = su; sv[8 + q4] = sq;
-                }
-#pragma unroll
-                for (int m = 16, half = 8; m >= 2; m >>= 1, half >>= 1) {
-                    const bool upper = (lane & m) != 0;
-#pragma unroll
-                    for (int i = 0; i < half; ++i) {
-                        const float send = upper ? sv[i] : sv[i + half];
-                        const float recv = __shfl_xor_sync(0xffffffffu, send, m);
-                        sv[i] = (upper ? sv[i + half] : sv[i]) + recv;
-                    }
-                }
-                sv[0] += __shfl_xor_sync(0xffffffffu, sv[0], 1);
-                if ((lane & 1) == 0) {
-                    const int idx = ((lane >> 4) & 1) * 8 + ((lane >> 3) & 1) * 4 + ((lane >> 2) & 1) * 2 + ((lane >> 1) & 1);
-                    atomicAdd(qacc + (c0 / 4 + (idx & 7)) * 2 + (idx >> 3), sv[0]);
-                }
-            }
-            if (it + 1 < kIts) {
-#pragma unroll
-                for (int g = 0; g < 4; ++g) rcur[g] = rnext[g];
-            }
-        }
-        tc_fence_before();
-        if (PAIR) mbar_arrive_cluster(mapa_u32(smem_u32(&tempty[acc]), 0)); else mbar_arrive(&tempty[acc]);
-        if (p.qstats) {
-            if (NW == 8) asm volatile("bar.sync 1, 256;" ::: "memory"); else asm volatile("bar.sync 1, 128;" ::: "memory");
-            const uint32_t et = threadIdx.x - 64;
-            if (et < 64) {
-                const float val = qacc[et];
-                if (val != 0.0f) atomicAdd(p.qstats + (size_t)b * 64 + et, val);
-                qacc[et] = 0.0f;
-            }
-            if (NW == 8) asm volatile("bar.sync 1, 256;" ::: "memory"); else asm volatile("bar.sync 1, 128;" ::: "memory");
-        }
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
+    for (int m = 4; m <= 16; m <<= 1) { su += __shfl_xor_sync(0xffffffffu, su, m); sq += __shfl_xor_sync(0xffffffffu, sq, m); }
 }
 
 }  // namespace ssdnerf

@@ -24,13 +24,12 @@ struct BitfieldLoader {
     __device__ __forceinline__ uint32_t operator()(uint32_t byte) const { return __ldg(g + byte); }
 };
 
-// one 32-byte texel (8 floats, 6 used) as ONE 256-bit read-only load (LDG.E.256, sm_100): half the load instructions and half the
-// L1 wavefronts of two 128-bit loads -- the gather is the main client of the L1 data pipe (profiles/r02_render_p_analysis.txt)
-struct Texel8 { float4 lo, hi; };
+// one 32-byte texel (8 floats, 6 used) as a 128-bit + a 64-bit read-only load of the same 32-byte sector (the widest loads sm_90 has)
+struct Texel8 { float4 lo; float2 hi; };
 __device__ __forceinline__ Texel8 ldg_texel8(const float* __restrict__ p) {
     Texel8 t;
-    asm("ld.global.nc.v8.f32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-        : "=f"(t.lo.x), "=f"(t.lo.y), "=f"(t.lo.z), "=f"(t.lo.w), "=f"(t.hi.x), "=f"(t.hi.y), "=f"(t.hi.z), "=f"(t.hi.w) : "l"(p));
+    t.lo = __ldg(reinterpret_cast<const float4*>(p));
+    t.hi = __ldg(reinterpret_cast<const float2*>(p + 4));
     return t;
 }
 
@@ -49,7 +48,8 @@ __device__ __forceinline__ void gather_plane_p(const float* __restrict__ plane, 
     const float nw = wx0 * wy0, ne = wx1 * wy0, sw = wx0 * wy1, se = wx1 * wy1;
     const Texel8 ta = ldg_texel8(plane + ((size_t)y0 * Wp + x0) * 8), tb = ldg_texel8(plane + ((size_t)y0 * Wp + x1) * 8);
     const Texel8 tc = ldg_texel8(plane + ((size_t)y1 * Wp + x0) * 8), td = ldg_texel8(plane + ((size_t)y1 * Wp + x1) * 8);
-    const float4 a0 = ta.lo, a1 = ta.hi, b0 = tb.lo, b1 = tb.hi, c0 = tc.lo, c1 = tc.hi, d0 = td.lo, d1 = td.hi;
+    const float4 a0 = ta.lo, b0 = tb.lo, c0 = tc.lo, d0 = td.lo;
+    const float2 a1 = ta.hi, b1 = tb.hi, c1 = tc.hi, d1 = td.hi;
     f[0] = a0.x * nw + b0.x * ne + c0.x * sw + d0.x * se;
     f[1] = a0.y * nw + b0.y * ne + c0.y * sw + d0.y * se;
     f[2] = a0.z * nw + b0.z * ne + c0.z * sw + d0.z * se;

@@ -115,7 +115,7 @@ __global__ void __launch_bounds__(kDenThreads) k_density_update_p(const float* _
 // One warp per group of 32 voxels; lane = voxel for the gather (fp16 planes, same arithmetic as the S renderer), the 96 -> 128
 // base layer runs on the CUDA cores with fp32 accumulation: W1 is staged once per CTA in shared memory as fp32 [k][n] so that a
 // warp reads one broadcast float4 per 4 hidden units.  The grid builder is ~1 % of a step; simplicity over speed here.
-struct DecSOff {   // blob offsets of render_tc.cu::DecS
+struct DecSOff {   // blob offsets of render_common.cuh::DecS
     static constexpr int KF = 96, HID = 128, OFF_W1 = 0, OFF_B1 = HID * KF, OFF_WD = OFF_B1 + HID, OFF_BD = OFF_WD + HID;
 };
 
@@ -209,7 +209,7 @@ __global__ void __launch_bounds__(kDenThreads) k_density_update_s(const __half* 
         for (int n = 0; n < 128; ++n) {
             const float h = 0.5f * acc[n];
             float th; asm("tanh.approx.f32 %0, %1;" : "=f"(th) : "f"(h));
-            sd = fmaf(__half2float(__float2half_rn(fmaf(h, th, h))), wd[n], sd);       // SiLU as in render_tc.cu, fp16 operand
+            sd = fmaf(__half2float(__float2half_rn(fmaf(h, th, h))), wd[n], sd);       // SiLU as in render_s2.cu, fp16 operand
         }
         const float sigma = __expf(sd);
         const size_t gi = (size_t)scene * G3 + morton3D(i, j, k);
@@ -299,8 +299,8 @@ int ssdnerf_density_update(int variant, const void* planes, uint32_t plane_h, ui
                            uint32_t num_scenes, uint32_t grid_size, float bound, const float* jitter, float decay,
                            void* density_grid, int grid_is_half, void* workspace, void* stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
-    const bool is_s = variant == SSDNERF_DEC_S || variant == SSDNERF_DEC_S_MMA || variant == SSDNERF_DEC_S_TC;
-    if (!is_s && variant != SSDNERF_DEC_P && variant != SSDNERF_DEC_P_SIMT && variant != SSDNERF_DEC_P_TC && variant != SSDNERF_DEC_P_MMA && variant != SSDNERF_DEC_P_MMA2)
+    const bool is_s = variant == SSDNERF_DEC_S || variant == SSDNERF_DEC_S_MMA;
+    if (!is_s && variant != SSDNERF_DEC_P && variant != SSDNERF_DEC_P_SIMT && variant != SSDNERF_DEC_P_MMA && variant != SSDNERF_DEC_P_MMA2)
         return set_error_msg(SSDNERF_ERR_ARG, "density_update: unknown decoder variant");
     if (!planes || !decoder_blob || !density_grid || !workspace) return set_error_msg(SSDNERF_ERR_ARG, "density_update: NULL argument");
     if (grid_size == 0 || grid_size > 1024 || (grid_size & (grid_size - 1))) return set_error_msg(SSDNERF_ERR_ARG, "density_update: grid_size must be a power of two");

@@ -1,4 +1,4 @@
-// Persistent, warp-specialised tcgen05 GEMM / implicit-GEMM convolution for the UNet of the DDIM loop.
+// Persistent, warp-specialised wgmma GEMM / implicit-GEMM convolution for the UNet of the DDIM loop.
 //
 //   D[m, n] = alpha * sum_{tap, k} A_tap[m, k] * B[tap][n, k]  (+ bias[n]) (+ residual[m, n])
 //
@@ -7,16 +7,17 @@
 //   hardware's out-of-bounds zero fill supplying the padding (no im2col buffer).  A plain / batched GEMM is
 //   the same kernel with taps = 1.  A may be split along K over two tensors (UNet skip concat).
 // * B (weights [taps][N][K] or a batched operand) is K-major too; both land in 128B-swizzled smem tiles.
-// * tcgen05.mma (M=128, N=BN, K=16, fp16 x fp16 -> fp32) accumulates in TMEM; accumulators are double
-//   buffered so the epilogue of tile i overlaps the main loop of tile i+1.
-// * warp 0 = TMA producer, warp 1 = MMA issuer (+ TMEM owner; converged warp, elected lane), warps 2..9 = epilogue
-//   (TMEM -> regs -> bias / residual / GroupNorm quad statistics -> staged 64-byte row pieces -> global).
-// * cluster modes (CL): CTA pair with tcgen05.mma.cta_group::2 (auto for N = 256 tiles), multicast clusters of 4 / 8 (kept for A/B).
+// * warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 = consumers: each owns 64 of the tile's 128 rows and accumulates
+//   64 x BN fp32 in registers with wgmma.mma_async (m64nBNk16, fp16 x fp16 -> fp32, both operands from shared memory), then runs the
+//   epilogue (bias / residual / GroupNorm quad statistics / store) straight from the accumulator fragments while the producer already
+//   fills the stages of the next tile.
+// * clusters of CL = 2 / 4 / 8 CTAs along M: each CTA fetches 1/CL of the B (weight) tile and TMA-multicasts it to the whole cluster.
 //
 // Replaces on the reference path: cuDNN Conv2d 3x3/1x1, Conv1d qkv/proj and the attention einsums of
 // lib/models/architecture/ddpm/{denoising,modules}.py (+ mmgen 0.7.2 blocks), see ssdnerf_b200/unet.py.
 #include "common.cuh"
 #include "tc_common.cuh"
+#include "conv_row_epilogue.cuh"
 #include "../../include/ssdnerf_b200.h"
 #include <cuda_fp16.h>
 #include <cstdio>
@@ -24,8 +25,7 @@
 namespace ssdnerf {
 using namespace tc;
 
-constexpr int kGemmThreads = 320;      // warp 0 TMA, warp 1 MMA, warps 2..9 epilogue (two warps per TMEM lane quarter)
-constexpr int kEpiThreads = 256;
+constexpr int kGemmThreads = 384;      // warpgroup 0 TMA producer, warpgroups 1..2 wgmma consumers + epilogue
 constexpr int kMaxBiasN = 2048;         // bias vector staged in shared memory once per CTA
 constexpr int kBM = 128, kBK = 64;
 constexpr int kABytes = kBM * kBK * 2;  // 16 KB
@@ -41,6 +41,7 @@ struct GemmParams {
     uint32_t kc1, kc2;          // 64-wide K chunks taken from A1 / A2 per tap
     uint32_t n_valid;           // output columns
     uint32_t b_batched;         // B coords (c2, c3) = (t2, t3) instead of (tap, 0)
+    uint32_t vec2;              // output / residual element pairs are 4-byte (fp16) / 8-byte (fp32) aligned: paired stores
     float alpha;
     const float* bias_n;
     const __half* residual;
@@ -50,34 +51,23 @@ struct GemmParams {
     float* qstats;              // optional [images][n_valid/4][2]: per-image sum / sum-of-squares of every 4-channel quad of the output
     uint32_t stats_hw;          // > 0: image index of a row = (row index along d1) / stats_hw; 0: image index = index along d3
     unsigned long long* prof;   // optional debug counters (clock cycles summed over CTAs): [0] producer wait-empty, [1] producer total,
-                                // [2] MMA wait-full, [3] MMA wait-tmem-empty, [4] MMA total, [5] epilogue wait-tmem-full, [6] epilogue total
+                                // [2] consumer wait-full (warpgroup 1), [4] consumer total (warpgroup 1)
 };
 
-// CL = cluster size and mode: 1 = single CTA; 2 = CTA pair (one M = 256 MMA over two SMs, each stages half of B);
-// 4 / 8 = multicast cluster (every CTA loads 1/CL of the B tile and multicasts it to all, own M = 128 MMAs)
+// CL = cluster size: 1 = single CTA; 2 / 4 / 8 = multicast cluster (every CTA loads 1/CL of the B tile and multicasts it to all)
 template <int BN, int CL>
 struct GemmCfg {
-    static constexpr bool kPair = (CL == 2);
-    static constexpr int kMC = (CL >= 4) ? CL : 1;
-    static constexpr int kBRows = kPair ? BN / 2 : BN;     // B rows resident per CTA and stage
-    static constexpr int kBoxRowsB = kPair ? BN / 2 : BN / kMC;   // B rows fetched by ONE TMA instruction of this CTA
-    static constexpr int kBBytes = kBRows * kBK * 2;
+    static constexpr int kBBytes = BN * kBK * 2;
+    static constexpr int kBoxRowsB = BN / CL;                // B rows fetched by ONE TMA instruction of this CTA
     static constexpr int kStageBytes = kABytes + kBBytes;
     static constexpr int kStages = (192 * 1024 / kStageBytes) > 8 ? 8 : (192 * 1024 / kStageBytes);
-    static constexpr uint32_t kTxBytes = (kPair ? 2u : 1u) * kStageBytes;   // bytes credited to the (pair: leader's) full barrier per stage
-    static constexpr int kTmemCols = (2 * BN < 32) ? 32 : 2 * BN;   // power of two for BN in {32,64,128,256}
     static constexpr size_t kSmem = (size_t)kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/ + 1024 /*quad-stat accumulators*/ +
-                                    kMaxBiasN * 4 /*bias*/ + 8 * 2048 /*epilogue transpose staging, 2 KB per warp*/;
+                                    kMaxBiasN * 4 /*bias*/;
 };
 
-// The large layers are bound by the chip-wide L2 -> SM operand bandwidth (~60 B/clk/SM when all SMs pull; profiles/r01_gemm_pipeline_*),
-// not by the tensor pipe: a 128 x BN tile re-fetches (128 + BN) x 128 B per 64-wide k-block.  Two ways to fetch less per flop:
-// CL = 4 / 8: the CL CTAs of a cluster work on CL consecutive M tiles of the same N tile; each fetches 1/CL of the B (weight) tile and
-//   TMA-multicasts it into every CTA's shared memory -> B traffic / CL (L2 de-duplicates by itself only up to ~4 concurrent readers).
-// CL = 2: CTA pair (two SMs of a TPC) on 2 consecutive M tiles of the same N tile with ONE tcgen05.mma.cta_group::2 of M = 256:
-// each CTA stages its own 128-row A tile and HALF of the B (weight) tile, the leader's MMA reads both halves, so the shared-memory
-// write + read traffic per SM and per MMA drops from A + B to A + B/2 -- the single-SM kernel is shared-memory-bandwidth bound
-// (an M = 128 MMA re-reads both operands every 64 (N = 128) / 128 (N = 256) cycles while TMA refills them).
+// The large layers are bound by operand delivery (L2 -> shared memory) rather than by the tensor cores: a 128 x BN tile re-fetches
+// (128 + BN) x 128 B per 64-wide k-block.  Wide N tiles (BN = 256, two consumer warpgroups of 64 x 256) amortise the A tile best;
+// multicast clusters additionally cut the B (weight) traffic by CL.
 template <int BN, int CL>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 k_gemm_tc(const __grid_constant__ CUtensorMap mapA1, const __grid_constant__ CUtensorMap mapA2,
@@ -89,46 +79,38 @@ k_gemm_tc(const __grid_constant__ CUtensorMap mapA1, const __grid_constant__ CUt
     uint8_t* sB = smem + Cfg::kStages * kABytes;
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
     uint64_t* empty = full + Cfg::kStages;
-    uint64_t* tfull = empty + Cfg::kStages;
-    uint64_t* tempty = tfull + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
     float* qacc = reinterpret_cast<float*>(smem + Cfg::kStages * Cfg::kStageBytes + 256);   // [2 images][BN/4][2]
     float* sbias = qacc + 256;                                                               // [kMaxBiasN]
-    uint8_t* sstage = reinterpret_cast<uint8_t*>(sbias + kMaxBiasN);                          // [8 warps][32 rows][64 B]
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
     const uint32_t tiles_m = p.T1 * p.T2 * p.T3;
     const uint32_t sup_m = (tiles_m + CL - 1) / CL;                 // super-tiles (CL M tiles) along M
     const uint32_t total_tiles = sup_m * p.tiles_n;                   // work items per cluster
     const uint32_t iters = p.taps * (p.kc1 + p.kc2);
-    constexpr bool kPair = Cfg::kPair;
-    constexpr int kMC = Cfg::kMC;
     const uint32_t crank = (CL > 1) ? cluster_ctarank() : 0u;
     const uint32_t tile0 = (CL > 1) ? cluster_id_x() : blockIdx.x;
     const uint32_t tile_step = (CL > 1) ? num_clusters_x() : gridDim.x;
     constexpr uint16_t kMask = (uint16_t)((1u << CL) - 1u);
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         prefetch_tmap(&mapA1); prefetch_tmap(&mapA2); prefetch_tmap(&mapB);
-        for (int i = 0; i < Cfg::kStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kMC); }   // multicast: every CTA's MMA releases the stage
-        for (int i = 0; i < 2; ++i) { mbar_init(&tfull[i], 1); mbar_init(&tempty[i], kEpiThreads * (kPair ? 2 : 1)); }   // pair: both epilogues free the leader's
+        // every consumer warp of every CTA of the cluster releases a stage (the multicast B slices land in all of them)
+        for (int i = 0; i < Cfg::kStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 8 * CL); }
         fence_mbar_init();
     }
-    if (warp == 1) { if (kPair) tmem_alloc2(tmem_slot, Cfg::kTmemCols); else tmem_alloc(tmem_slot, Cfg::kTmemCols); }
     for (int i = threadIdx.x; i < BN; i += kGemmThreads) qacc[i] = 0.0f;     // 2 * BN/4 * 2 floats
     if (p.bias_n) for (uint32_t i = threadIdx.x; i < p.n_valid; i += kGemmThreads) sbias[i] = __ldg(p.bias_n + i);
-    tc_fence_before();
     __syncthreads();
     if (CL > 1) cluster_sync_all();       // peers' barriers are initialised before any multicast load / remote arrive targets them
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    // everything above touched only shared memory, TMEM and constant weights (bias): it may overlap the tail of the preceding
-    // kernel; activations, residual, statistics and the output buffer are only touched after the dependency is resolved
+    // everything above touched only shared memory and constant weights (bias): it may overlap the tail of the preceding kernel;
+    // activations, residual, statistics and the output buffer are only touched after the dependency is resolved
     pdl_trigger();
     pdl_wait();
 
-    if (warp == 0) {
-        {   // ---------------- TMA producer: the whole warp runs the loop converged, one elected lane issues (see tc_common.cuh)
+    // register budget: setmaxnreg moves registers within the CTA's launch-time pool (384 x 168): 128 x 40 + 256 x 232 = 384 x 168
+    if (wg == 0) {
+        setmaxnreg_dec<40>();
+        if (threadIdx.x == 0) {   // ---------------- TMA producer
             uint32_t stage = 0, phase = 0;
             long long pw = 0; const long long pt0 = clock64();
             for (uint32_t tile = tile0; tile < total_tiles; tile += tile_step) {
@@ -141,245 +123,131 @@ k_gemm_tc(const __grid_constant__ CUtensorMap mapA1, const __grid_constant__ CUt
                         else mbar_wait(&empty[stage], phase ^ 1);
                         const bool first = j < p.kc1;
                         const int ak = (int)((first ? j : j - p.kc1) * kBK), a1 = (int)(t1 * p.b1 * p.a_stride) + ox, a2 = (int)(t2 * p.b2 * p.a_stride) + oy, a3 = (int)(t3 * p.b3);
+                        mbar_expect_tx(&full[stage], (uint32_t)Cfg::kStageBytes);
+                        tma_load_4d(sA + stage * kABytes, first ? &mapA1 : &mapA2, &full[stage], ak, a1, a2, a3);
                         if (CL == 1) {
-                            mbar_expect_tx_w(&full[stage], Cfg::kTxBytes);
-                            tma_load_4d_w(sA + stage * kABytes, first ? &mapA1 : &mapA2, &full[stage], ak, a1, a2, a3);
-                            tma_load_4d_w(sB + stage * Cfg::kBBytes, &mapB, &full[stage], (int)(j * kBK), (int)(n_tile * BN),
-                                          p.b_batched ? (int)t2 : (int)tap, p.b_batched ? (int)t3 : 0);
-                        } else if (kMC > 1) {   // own A tile + this CTA's 1/CL slice of the B tile broadcast to the whole cluster
-                            mbar_expect_tx_w(&full[stage], Cfg::kTxBytes);
-                            tma_load_4d_w(sA + stage * kABytes, first ? &mapA1 : &mapA2, &full[stage], ak, a1, a2, a3);
-                            tma_load_4d_mc_w(sB + stage * Cfg::kBBytes + crank * Cfg::kBoxRowsB * 128, &mapB, &full[stage], (int)(j * kBK),
-                                             (int)(n_tile * BN + crank * Cfg::kBoxRowsB), (int)tap, 0, kMask);
-                        } else {   // pair: own A tile + own half of the B tile, all bytes credited to the leader's barrier
-                            if (crank == 0) mbar_expect_tx_w(&full[stage], Cfg::kTxBytes);
-                            const uint32_t lbar = mapa_u32(smem_u32(&full[stage]), 0);
-                            tma_load_4d_2cta_w(sA + stage * kABytes, first ? &mapA1 : &mapA2, lbar, ak, a1, a2, a3);
-                            tma_load_4d_2cta_w(sB + stage * Cfg::kBBytes, &mapB, lbar, (int)(j * kBK), (int)(n_tile * BN + crank * Cfg::kBRows),
-                                               (int)tap, 0);
+                            tma_load_4d(sB + stage * Cfg::kBBytes, &mapB, &full[stage], (int)(j * kBK), (int)(n_tile * BN),
+                                        p.b_batched ? (int)t2 : (int)tap, p.b_batched ? (int)t3 : 0);
+                        } else {   // this CTA's 1/CL slice of the B tile, broadcast to the whole cluster
+                            tma_load_4d_mc(sB + stage * Cfg::kBBytes + crank * Cfg::kBoxRowsB * 128, &mapB, &full[stage], (int)(j * kBK),
+                                           (int)(n_tile * BN + crank * Cfg::kBoxRowsB), (int)tap, 0, kMask);
                         }
                         if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
                     }
                 }
             }
-            if (p.prof && lane == 0) { atomicAdd(p.prof + 0, (unsigned long long)pw); atomicAdd(p.prof + 1, (unsigned long long)(clock64() - pt0)); }
+            if (p.prof) { atomicAdd(p.prof + 0, (unsigned long long)pw); atomicAdd(p.prof + 1, (unsigned long long)(clock64() - pt0)); }
         }
-        __syncwarp();
-    } else if (warp == 1) {
-        if (!kPair || crank == 0) {   // ---------------- MMA issuer: converged warp, elected lane issues (pair: the leader CTA issues for both SMs)
-            constexpr uint32_t idesc = make_idesc_f16(kBM * (kPair ? 2 : 1), BN);
-            uint32_t stage = 0, phase = 0, acc = 0, acc_phase = 0;
-            long long wf = 0, we = 0; const long long mt0 = clock64();
-            for (uint32_t tile = tile0; tile < total_tiles; tile += tile_step) {
-                const long long c0 = p.prof ? clock64() : 0;
-                if (kPair) mbar_wait_cluster(&tempty[acc], acc_phase ^ 1); else mbar_wait(&tempty[acc], acc_phase ^ 1);
-                if (p.prof) we += clock64() - c0;
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + acc * BN;
-                for (uint32_t it = 0; it < iters; ++it) {
-                    if (p.prof) { const long long c = clock64(); mbar_wait(&full[stage], phase); wf += clock64() - c; }
-                    else mbar_wait(&full[stage], phase);
-                    tc_fence_after();
-                    const uint64_t a_desc = make_desc_sw128(smem_u32(sA + stage * kABytes));
-                    const uint64_t b_desc = make_desc_sw128(smem_u32(sB + stage * Cfg::kBBytes));
-#pragma unroll
-                    for (uint32_t k = 0; k < kBK / 16; ++k) {   // advance 16 halves = 32 B = 2 descriptor units along K
-                        if (kPair) umma_f16_2cta_w(d_tmem, a_desc + 2 * k, b_desc + 2 * k, idesc, (it | k) != 0);
-                        else umma_f16_w(d_tmem, a_desc + 2 * k, b_desc + 2 * k, idesc, (it | k) != 0);
-                    }
-                    if (kPair) umma_commit_2cta_w(&empty[stage], kMask);        // frees this stage in both CTAs
-                    else if (kMC > 1) umma_commit_mc_w(&empty[stage], kMask);   // one of the CL releases every CTA's producer waits for
-                    else umma_commit_w(&empty[stage]);
-                    if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-                }
-                if (kPair) umma_commit_2cta_w(&tfull[acc], kMask); else umma_commit_w(&tfull[acc]);
-                if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+    } else {   // ---------------- consumers: warpgroup cw owns rows 64 cw .. 64 cw + 63 of every tile
+        setmaxnreg_inc<232>();
+        const uint32_t cw = (uint32_t)wg - 1u;
+        const uint32_t wq = (uint32_t)warp & 3u;
+        const uint32_t rbase = cw * 64u + wq * 16u + ((uint32_t)lane >> 2);     // this thread's rows: rbase, rbase + 8
+        const uint32_t cq = (uint32_t)lane & 3u;
+        uint32_t stage = 0, phase = 0;
+        long long wf = 0; const long long ct0 = clock64();
+        float acc[BN / 2];
+        auto release = [&](uint32_t s) {
+            if (lane == 0) {
+                if (CL == 1) mbar_arrive(&empty[s]);
+                else for (uint32_t r = 0; r < (uint32_t)CL; ++r) mbar_arrive_cluster(mapa_u32(smem_u32(&empty[s]), r));
             }
-            if (p.prof && lane == 0) {
-                atomicAdd(p.prof + 2, (unsigned long long)wf); atomicAdd(p.prof + 3, (unsigned long long)we);
-                atomicAdd(p.prof + 4, (unsigned long long)(clock64() - mt0));
-            }
-        }
-        __syncwarp();
-    } else {   // ---------------- epilogue warps 2..9: TMEM lane quarter = warp % 4, column half = (warp - 2) / 4
-        const uint32_t q = (uint32_t)warp & 3u;
-        const uint32_t hsel = (uint32_t)(warp - 2) >> 2;
-        constexpr int kChunks = BN / 64;                     // 32-column chunks per warp
-        const uint32_t row = q * 32 + (uint32_t)lane;
-        const uint32_t i1 = row % p.b1, i2 = (row / p.b1) % p.b2, i3 = row / (p.b1 * p.b2);
-        const bool has_bias = p.bias_n != nullptr;
-        uint32_t acc = 0, acc_phase = 0;
-        long long ew = 0; const long long et0 = clock64();
+        };
         for (uint32_t tile = tile0; tile < total_tiles; tile += tile_step) {
             const uint32_t m_tile = (tile % sup_m) * CL + crank, n_tile = tile / sup_m;
             const uint32_t t1 = m_tile % p.T1, t2 = (m_tile / p.T1) % p.T2, t3 = m_tile / (p.T1 * p.T2);
-            const uint32_t g1 = t1 * p.b1 + i1, g2 = t2 * p.b2 + i2, g3 = t3 * p.b3 + i3;
-            const bool row_ok = m_tile < tiles_m && g1 < p.d1 && g2 < p.d2 && g3 < p.d3;
-            const long long off = (long long)g1 * p.so1 + (long long)g2 * p.so2 + (long long)g3 * p.so3 + (long long)n_tile * BN;
-            // GroupNorm quad statistics: image of this thread's row (warp-uniform) relative to the image of the tile's first row
-            const uint32_t img = p.stats_hw ? g1 / p.stats_hw : g3;
-            const uint32_t img0 = p.stats_hw ? (t1 * p.b1) / p.stats_hw : t3 * p.b3;
-            const uint32_t slot = (img - img0) & 1u;
-            const uint32_t cbeg = hsel * (BN / 2);
-            // Global accesses of the epilogue are re-mapped through a 2 KB per-warp staging tile so that one warp instruction touches
-            // 8 rows x 64 contiguous bytes (4 lanes per row) instead of 32 rows x 16 bytes: a row-per-lane 16-byte access costs 32 LSU
-            // wavefronts and made every short-K GEMM epilogue-bound (~2.7 k cycles per 32-column chunk, profiles/r01_gemm_pipeline_prof.txt).
-            const uint32_t wst = smem_u32(sstage) + (uint32_t)(warp - 2) * 2048u;     // shared-space address of this warp's staging tile
-            const uint32_t pc = (uint32_t)lane & 3u;
-            uint32_t st_own[4], st_map[4];     // swizzled byte offsets: own row (lane) piece g / re-mapped row (lane >> 2) + 8 i piece pc
 #pragma unroll
-            for (int g = 0; g < 4; ++g) {
-                st_own[g] = wst + (uint32_t)lane * 64u + (((uint32_t)g ^ (((uint32_t)lane >> 1) & 3u)) << 4);
-                const uint32_t r = ((uint32_t)lane >> 2) + 8u * g;
-                st_map[g] = wst + r * 64u + ((pc ^ ((r >> 1) & 3u)) << 4);
-            }
-            long long roff[4]; bool rok[4];            // rows (lane >> 2) + 8 i of this warp's 32-row slice, as seen by the re-mapped accesses
+            for (int i = 0; i < BN / 2; ++i) acc[i] = 0.0f;
+            uint32_t prev = 0;
+            for (uint32_t it = 0; it < iters; ++it) {
+                if (p.prof && cw == 0) { const long long c = clock64(); mbar_wait(&full[stage], phase); wf += clock64() - c; }
+                else mbar_wait(&full[stage], phase);
+                const uint64_t a_desc = make_desc_sw128(smem_u32(sA + stage * kABytes + cw * 64 * 128));
+                const uint64_t b_desc = make_desc_sw128(smem_u32(sB + stage * Cfg::kBBytes));
+                wgmma_fence();
+                fence_regs(acc);
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const uint32_t rr = q * 32 + ((uint32_t)lane >> 2) + 8u * i;
-                const uint32_t j1 = rr % p.b1, j2 = (rr / p.b1) % p.b2, j3 = rr / (p.b1 * p.b2);
-                const uint32_t h1 = t1 * p.b1 + j1, h2 = t2 * p.b2 + j2, h3 = t3 * p.b3 + j3;
-                rok[i] = m_tile < tiles_m && h1 < p.d1 && h2 < p.d2 && h3 < p.d3;
-                roff[i] = (long long)h1 * p.so1 + (long long)h2 * p.so2 + (long long)h3 * p.so3 + (long long)n_tile * BN;
-            }
-            // the residual does not depend on the accumulator: its loads are issued before the wait on the MMA (and one chunk ahead)
-            uint4 rcur[4], rnext[4];
-            auto fetch_res = [&](uint32_t c0, uint4* r) {
-                const bool full = p.residual && (n_tile * BN + c0 + 32 <= p.n_valid);          // warp-uniform
-#pragma unroll
-                for (int i = 0; i < 4; ++i)
-                    r[i] = (full && rok[i]) ? __ldg(reinterpret_cast<const uint4*>(p.residual + roff[i] + c0 + pc * 8)) : make_uint4(0, 0, 0, 0);
-            };
-            fetch_res(cbeg, rcur);
-            if (p.prof) { const long long c = clock64(); mbar_wait(&tfull[acc], acc_phase); ew += clock64() - c; }
-            else mbar_wait(&tfull[acc], acc_phase);
-            tc_fence_after();
-#pragma unroll
-            for (int ci = 0; ci < kChunks; ++ci) {
-                const uint32_t c0 = cbeg + 32u * ci;
-                uint32_t v[32];
-                tmem_ld32(tmem_base + ((q * 32u) << 16) + acc * BN + c0, v);
-                if (ci + 1 < kChunks) fetch_res(c0 + 32, rnext);
-                const uint32_t ncol0 = n_tile * BN + c0;
-                const bool full32 = (ncol0 + 32 <= p.n_valid);                                  // warp-uniform
-                uint4 rrow[4];                                                                  // this lane's own row of the residual
-                if (p.residual && full32) {
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) sts128(st_map[i], rcur[i]);
-                    __syncwarp();
-#pragma unroll
-                    for (int g = 0; g < 4; ++g) rrow[g] = lds128(st_own[g]);
-                    __syncwarp();
+                for (uint32_t k = 0; k < kBK / 16; ++k) {   // advance 16 halves = 32 B = 2 descriptor units along K
+                    if constexpr (BN == 256) wgmma_ss_n256(acc, a_desc + 2 * k, b_desc + 2 * k, 1u);
+                    else if constexpr (BN == 128) wgmma_ss_n128(acc, a_desc + 2 * k, b_desc + 2 * k, 1u);
+                    else wgmma_ss_n64(acc, a_desc + 2 * k, b_desc + 2 * k, 1u);
                 }
-                tmem_ld_wait();
-                float f[32];
-                const bool live = row_ok && ncol0 < p.n_valid;      // rows / columns outside the problem: f is never stored and masked out of the statistics
-                if (p.alpha != 1.0f) {
+                wgmma_commit();
+                fence_regs(acc);
+                wgmma_wait<1>();                          // the previous k-block's MMAs are done: its stage goes back to the producer
+                if (it > 0) release(prev);
+                prev = stage;
+                if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+            }
+            wgmma_wait<0>();
+            fence_regs(acc);
+            if (iters > 0) release(prev);
+
+            // ---------------- epilogue from the accumulator fragments: rows rbase + 8 h, columns 8 i + 2 cq + e
+            long long off[2]; bool rok[2];
 #pragma unroll
-                    for (int i = 0; i < 32; ++i) f[i] = __uint_as_float(v[i]) * p.alpha;
-                } else {
+            for (int h = 0; h < 2; ++h) {
+                const uint32_t row = rbase + 8u * h;
+                const uint32_t i1 = row % p.b1, i2 = (row / p.b1) % p.b2, i3 = row / (p.b1 * p.b2);
+                const uint32_t g1 = t1 * p.b1 + i1, g2 = t2 * p.b2 + i2, g3 = t3 * p.b3 + i3;
+                rok[h] = m_tile < tiles_m && g1 < p.d1 && g2 < p.d2 && g3 < p.d3;
+                off[h] = (long long)g1 * p.so1 + (long long)g2 * p.so2 + (long long)g3 * p.so3 + (long long)n_tile * BN;
+            }
+            // GroupNorm quad statistics: rows of one 64-row half of a tile belong to one image (b1 * b2 * b3 = 128 are powers of two and
+            // stats_hw is a multiple of 64), the slot is that image relative to the image of the tile's first row
+            uint32_t slot = 0, img0 = 0;
+            if (p.qstats) {
+                const uint32_t r0 = cw * 64u;
+                const uint32_t j1 = r0 % p.b1, j3 = r0 / (p.b1 * p.b2);
+                img0 = p.stats_hw ? (t1 * p.b1) / p.stats_hw : t3 * p.b3;
+                slot = ((p.stats_hw ? (t1 * p.b1 + j1) / p.stats_hw : t3 * p.b3 + j3) - img0) & 1u;
+            }
 #pragma unroll
-                    for (int i = 0; i < 32; ++i) f[i] = __uint_as_float(v[i]);
-                }
-                if (live) {
-                    if (has_bias) {
-                        if (full32) {
+            for (int i = 0; i < BN / 8; ++i) {
+                const uint32_t c0 = 8u * i + 2u * cq;                  // column within the tile
+                const uint32_t ncol = n_tile * BN + c0;
+                const bool okc0 = ncol < p.n_valid, okc1 = ncol + 1 < p.n_valid;
+                float su = 0.0f, sq = 0.0f;
 #pragma unroll
-                            for (int g = 0; g < 8; ++g) {
-                                const float4 b = *reinterpret_cast<const float4*>(sbias + ncol0 + 4 * g);
-                                f[4 * g] += b.x; f[4 * g + 1] += b.y; f[4 * g + 2] += b.z; f[4 * g + 3] += b.w;
-                            }
-                        } else {
-#pragma unroll
-                            for (int i = 0; i < 32; ++i) if (ncol0 + i < p.n_valid) f[i] += sbias[ncol0 + i];
-                        }
-                    }
+                for (int h = 0; h < 2; ++h) {
+                    float v0 = acc[4 * i + 2 * h] * p.alpha, v1 = acc[4 * i + 2 * h + 1] * p.alpha;
+                    if (!rok[h] || !okc0) continue;
+                    if (p.bias_n) { v0 += sbias[ncol]; if (okc1) v1 += sbias[ncol + 1]; }
+                    const long long o = off[h] + c0;
                     if (p.residual) {
-                        if (full32) {
-#pragma unroll
-                            for (int g = 0; g < 4; ++g) {
-                                const __half2* h2 = reinterpret_cast<const __half2*>(&rrow[g]);
-#pragma unroll
-                                for (int i = 0; i < 4; ++i) { const float2 t = __half22float2(h2[i]); f[8 * g + 2 * i] += t.x; f[8 * g + 2 * i + 1] += t.y; }
-                            }
+                        if (p.vec2 && okc1) {
+                            const float2 r = __half22float2(*reinterpret_cast<const __half2*>(p.residual + o));
+                            v0 += r.x; v1 += r.y;
                         } else {
-                            const __half* rp = p.residual + off + c0;
-                            for (int i = 0; i < 32; ++i) if (ncol0 + i < p.n_valid) f[i] += __half2float(rp[i]);
+                            v0 += __half2float(p.residual[o]);
+                            if (okc1) v1 += __half2float(p.residual[o + 1]);
                         }
                     }
-                }
-                if (!p.out_f32 && full32) {          // fp16 rows through the staging tile (warp-uniform branch)
-#pragma unroll
-                    for (int g = 0; g < 4; ++g) {
-                        uint4 o;
-                        __half2* h2 = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) h2[i] = __floats2half2_rn(f[8 * g + 2 * i], f[8 * g + 2 * i + 1]);
-                        sts128(st_own[g], o);
-                    }
-                    __syncwarp();
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        const uint4 o = lds128(st_map[i]);
-                        if (rok[i]) *reinterpret_cast<uint4*>(reinterpret_cast<__half*>(p.out) + roff[i] + c0 + pc * 8) = o;
-                    }
-                    __syncwarp();
-                } else if (live) {
                     if (p.out_f32) {
-                        float* op = reinterpret_cast<float*>(p.out) + off + c0;
-                        if (full32) {
-#pragma unroll
-                            for (int g = 0; g < 8; ++g) reinterpret_cast<float4*>(op)[g] = make_float4(f[4 * g], f[4 * g + 1], f[4 * g + 2], f[4 * g + 3]);
-                        } else {
-                            for (int i = 0; i < 32; ++i) if (ncol0 + i < p.n_valid) op[i] = f[i];
-                        }
+                        float* op = reinterpret_cast<float*>(p.out) + o;
+                        if (p.vec2 && okc1) *reinterpret_cast<float2*>(op) = make_float2(v0, v1);
+                        else { op[0] = v0; if (okc1) op[1] = v1; }
                     } else {
-                        __half* op = reinterpret_cast<__half*>(p.out) + off + c0;
-                        for (int i = 0; i < 32; ++i) if (ncol0 + i < p.n_valid) op[i] = __float2half_rn(f[i]);
+                        __half* op = reinterpret_cast<__half*>(p.out) + o;
+                        if (p.vec2 && okc1) *reinterpret_cast<__half2*>(op) = __floats2half2_rn(v0, v1);
+                        else { op[0] = __float2half_rn(v0); if (okc1) op[1] = __float2half_rn(v1); }
                     }
+                    if (!okc1) v1 = 0.0f;
+                    su += v0 + v1; sq = fmaf(v0, v0, fmaf(v1, v1, sq));
                 }
-                if (p.qstats) {   // fused GroupNorm statistics of the fp32 output values: 8 quads x {sum, sumsq} per thread ...
-                    float sv[16];
-#pragma unroll
-                    for (int q4 = 0; q4 < 8; ++q4) {
-                        float su = 0.0f, sq = 0.0f;
-#pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            float x = f[4 * q4 + e];
-                            if (!live || ncol0 + 4 * q4 + e >= p.n_valid) x = 0.0f;
-                            su += x; sq = fmaf(x, x, sq);
-                        }
-                        sv[q4] = su; sv[8 + q4] = sq;
+                if (p.qstats) {
+                    frag_quad_reduce(su, sq);
+                    if ((lane & ~2) == 0) {                                // lanes 0 / 2: quads 2 i / 2 i + 1 of the tile over this warp's 16 rows
+                        float* qa = qacc + (slot * (BN / 4) + 2 * i + (lane >> 1)) * 2;
+                        atomicAdd(qa, su); atomicAdd(qa + 1, sq);
                     }
-                    // ... reduce-scattered over the warp's 32 rows with 16 shuffles: lane bits 4..1 select which of the 16 values it ends with
-#pragma unroll
-                    for (int m = 16, half = 8; m >= 2; m >>= 1, half >>= 1) {
-                        const bool upper = (lane & m) != 0;
-#pragma unroll
-                        for (int i = 0; i < half; ++i) {
-                            const float send = upper ? sv[i] : sv[i + half];
-                            const float recv = __shfl_xor_sync(0xffffffffu, send, m);
-                            sv[i] = (upper ? sv[i + half] : sv[i]) + recv;
-                        }
-                    }
-                    sv[0] += __shfl_xor_sync(0xffffffffu, sv[0], 1);
-                    if ((lane & 1) == 0) {
-                        const int idx = ((lane >> 4) & 1) * 8 + ((lane >> 3) & 1) * 4 + ((lane >> 2) & 1) * 2 + ((lane >> 1) & 1);
-                        atomicAdd(qacc + (slot * (BN / 4) + c0 / 4 + (idx & 7)) * 2 + (idx >> 3), sv[0]);
-                    }
-                }
-                if (ci + 1 < kChunks) {
-#pragma unroll
-                    for (int g = 0; g < 4; ++g) rcur[g] = rnext[g];
                 }
             }
-            tc_fence_before();
-            if (kPair) mbar_arrive_cluster(mapa_u32(smem_u32(&tempty[acc]), 0)); else mbar_arrive(&tempty[acc]);
             if (p.qstats) {
                 asm volatile("bar.sync 1, 256;" ::: "memory");
-                const uint32_t et = threadIdx.x - 64;                 // 0..255 within the epilogue warps
+                const uint32_t et = threadIdx.x - 128;                // 0..255 within the consumer warpgroups
                 const uint32_t nq = p.n_valid / 4;
-                for (uint32_t i = et; i < (uint32_t)BN; i += kEpiThreads) {   // i = (slot * BN/4 + quad) * 2 + stat
+                for (uint32_t i = et; i < (uint32_t)BN; i += 256) {     // i = (slot * BN/4 + quad) * 2 + stat
                     const float val = qacc[i];
                     const uint32_t sl = i / (BN / 2), qd = (i % (BN / 2)) >> 1, st = i & 1u;
                     const uint32_t gq = n_tile * (BN / 4) + qd;
@@ -388,14 +256,11 @@ k_gemm_tc(const __grid_constant__ CUtensorMap mapA1, const __grid_constant__ CUt
                 }
                 asm volatile("bar.sync 1, 256;" ::: "memory");
             }
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
         }
-        if (p.prof && threadIdx.x == 64) { atomicAdd(p.prof + 5, (unsigned long long)ew); atomicAdd(p.prof + 6, (unsigned long long)(clock64() - et0)); }
+        if (p.prof && threadIdx.x == 128) { atomicAdd(p.prof + 2, (unsigned long long)wf); atomicAdd(p.prof + 4, (unsigned long long)(clock64() - ct0)); }
     }
-    tc_fence_before();
     __syncthreads();
-    if (CL > 1) cluster_sync_all();       // nobody exits while a peer may still multicast into its shared memory
-    if (warp == 1) { tc_fence_after(); if (kPair) tmem_dealloc2(tmem_base, Cfg::kTmemCols); else tmem_dealloc(tmem_base, Cfg::kTmemCols); }
+    if (CL > 1) cluster_sync_all();       // nobody exits while a peer may still multicast into its shared memory or arrive on its barriers
 }
 
 // ---------------------------------------------------------------- host side: tensor maps
@@ -464,11 +329,11 @@ static int launch_gemm(const CUtensorMap& mA1, const CUtensorMap& mA2, const CUt
     at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[1].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
     cfg.attrs = at; cfg.numAttrs = 2;
-    static int max_clusters_dev[64] = {};     // co-resident clusters of this instantiation (1 CTA / SM; GPC sizes limit clusters of 4 / 8)
+    static int max_clusters_dev[64] = {};     // co-resident clusters of this instantiation (1 CTA / SM; GPC sizes limit clusters)
     int& max_clusters_cached = max_clusters_dev[current_device()];
     if (!max_clusters_cached) {
         max_clusters_cached = sms / CL;
-        if (CL > 2) {
+        if (CL > 1) {
             cfg.gridDim = dim3((uint32_t)(sms / CL) * CL);
             int n = 0;
             cfg.numAttrs = 1;
@@ -512,8 +377,8 @@ extern "C" int ssdnerf_gemm_f16(const ssdnerf_gemm_args* a, void* stream_) {
     if (a->algo == 2) return set_error_msg(SSDNERF_ERR_ARG, "gemm: algo 2 (row-pair convolution) needs taps 9, 128-pixel rows, 128 output channels, fp16 output");
     int bn = (int)a->bn;
     if (!bn) {
-        // pick the N tile that minimises (waves x tile cost): wide tiles amortise A loads (N=256 runs the MMA pipe at full rate,
-        // N=128 is shared-memory-bandwidth limited, N=64 more so) but small problems need more tiles to fill 148 SMs
+        // pick the N tile that minimises (waves x tile cost): wide tiles amortise A loads (a 64 x 256 wgmma per consumer warpgroup
+        // keeps the tensor cores busiest, N=128 and N=64 re-read A more often) but small problems need more tiles to fill every SM
         const uint32_t tiles_m = div_up(a->d1, a->b1) * div_up(a->d2, a->b2) * div_up(a->d3, a->b3);
         double best = 1e30;
         const int cand[3] = {256, 128, 64};
@@ -526,7 +391,6 @@ extern "C" int ssdnerf_gemm_f16(const ssdnerf_gemm_args* a, void* stream_) {
         }
     }
     if (bn != 64 && bn != 128 && bn != 256) return set_error_msg(SSDNERF_ERR_ARG, "gemm: bn must be 64, 128 or 256");
-    if (a->residual && a->out_f32 == 0 && a->residual == a->out) { /* in-place residual add is fine: same thread reads then writes */ }
 
     GemmParams p{};
     p.b1 = a->b1; p.b2 = a->b2; p.b3 = a->b3; p.d1 = a->d1; p.d2 = a->d2; p.d3 = a->d3;
@@ -542,6 +406,9 @@ extern "C" int ssdnerf_gemm_f16(const ssdnerf_gemm_args* a, void* stream_) {
     p.alpha = a->alpha; p.bias_n = a->bias_n; p.residual = (const __half*)a->residual; p.out = a->out; p.out_f32 = a->out_f32;
     p.so1 = a->so1; p.so2 = a->so2; p.so3 = a->so3;
     p.qstats = a->qstats; p.stats_hw = a->stats_hw; p.prof = (unsigned long long*)a->debug_cycles;
+    // element pairs (2 n, 2 n + 1) of a row are stored / read as one 4-byte (fp16) or 8-byte (fp32) access when every row offset is even
+    const uintptr_t pair_align = a->out_f32 ? 8u : 4u;
+    p.vec2 = ((a->so1 | a->so2 | a->so3) & 1) == 0 && ((uintptr_t)a->out % pair_align) == 0 && ((uintptr_t)a->residual & 3u) == 0;
     if (a->bias_n && a->n > (uint32_t)kMaxBiasN) return set_error_msg(SSDNERF_ERR_ARG, "gemm: bias vectors longer than 2048 are not supported");
     if (a->qstats && (a->n % 4)) return set_error_msg(SSDNERF_ERR_ARG, "gemm: quad statistics need n % 4 == 0");
     if (a->qstats && !a->stats_hw && a->b3 > 2) return set_error_msg(SSDNERF_ERR_ARG, "gemm: fused quad statistics cover at most 2 images per 128-row tile (b3 <= 2)");
@@ -557,14 +424,11 @@ extern "C" int ssdnerf_gemm_f16(const ssdnerf_gemm_args* a, void* stream_) {
     } else {
         mA2 = mA1;
     }
-    // clusters along M (weights shared): only for non-batched B.  The operand pipeline is latency-bound (shared-memory stages x bytes per
-    // stage / ~3300-cycle load round trip, profiles/r01_gemm_pipeline_*): what helps is more flops per staged byte, i.e. the CTA pair with
-    // N = 256 (each SM stages 128 + 128 rows for a 256 x 256 x 64 product); multicast clusters cut L2 traffic but not staged bytes and
-    // measured slower.  auto = pair for N = 256 tiles with >= 2 waves of M tiles.
-    const uint32_t tiles_m_all = p.T1 * p.T2 * p.T3;
-    int cl = (!a->b_batched && a->cluster == 0 && bn == 256 && tiles_m_all * p.tiles_n >= 2u * (uint32_t)sms) ? 2 : 1;
+    // clusters along M (weights shared, multicast B slices): only for non-batched B and on request; multicast cuts L2 traffic but not
+    // the staged bytes per SM, so auto stays with single CTAs
+    int cl = 1;
     if ((a->cluster == 2 || a->cluster == 4 || a->cluster == 8) && !a->b_batched && bn >= 128) cl = (int)a->cluster;
-    // B: {K, N, x2, x3}; box {64, rows fetched per TMA instruction (bn: single CTA, bn / 2: pair, bn / cl: multicast slice), 1, 1}
+    // B: {K, N, x2, x3}; box {64, rows fetched per TMA instruction (bn: single CTA, bn / cl: multicast slice), 1, 1}
     if (int e = make_map_4d(&mB, a->b, ktot, a->n_rows_b ? a->n_rows_b : a->n, a->bx2 ? a->bx2 : 1, a->bx3 ? a->bx3 : 1, a->b_strides[0],
                             a->b_strides[1], a->b_strides[2], (uint32_t)(bn / cl), 1, 1)) return e;
 

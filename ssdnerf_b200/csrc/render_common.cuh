@@ -1,4 +1,5 @@
-// Parameters and ray set-up shared by the fused render kernels (variant P: render_fused.cu, variant S: render_tc.cu).
+// Parameters and ray set-up shared by the fused render kernels (variant P: render_fused.cu / render_p2.cu / render_p3.cu,
+// variant S: render_s2.cu).
 #pragma once
 #include "common.cuh"
 
@@ -61,9 +62,6 @@ __device__ __forceinline__ void make_ray(const RenderParams& p, uint32_t scene, 
     r.rdx = __fdiv_rn(1.0f, r.dx); r.rdy = __fdiv_rn(1.0f, r.dy); r.rdz = __fdiv_rn(1.0f, r.dz);
 }
 
-// variant P on tensor cores (render_ptc.cu)
-int render_ptc_launch(const RenderParams& p, int emulate_schedule, uint32_t* hist, int sms, cudaStream_t stream);
-
 // variant P, warp-level mma.sync (render_p2.cu)
 int render_p2_launch(const RenderParams& p, int emulate_schedule, uint32_t* hist, int sms, cudaStream_t stream);
 
@@ -73,9 +71,13 @@ int render_p3_launch(const RenderParams& p, int emulate_schedule, uint32_t* hist
 // variant S, warp-level mma.sync (render_s2.cu)
 int render_s2_launch(const RenderParams& p, int emulate_schedule, uint32_t* hist, int sms, cudaStream_t stream);
 
-// variant S (render_tc.cu)
-size_t dec_s_blob_floats();
-int render_s_launch(const RenderParams& p, int emulate_schedule, uint32_t* hist, int sms, cudaStream_t stream);
+// variant S decoder blob (floats): W1[128][96] | b1[128] | Wd[128] | bd,0,0,0 | Wc0[128][144] | bc0[128] | Wc2[3][128] | bc2[3],0 | sat,0,0,0
+struct DecS {
+    static constexpr int C = 32, KF = 96, HID = 128, K2 = 144, N2 = 144;
+    static constexpr int OFF_W1 = 0, OFF_B1 = OFF_W1 + HID * KF, OFF_WD = OFF_B1 + HID, OFF_BD = OFF_WD + HID,
+                         OFF_WC0 = OFF_BD + 4, OFF_BC0 = OFF_WC0 + HID * K2, OFF_WC2 = OFF_BC0 + HID,
+                         OFF_BC2 = OFF_WC2 + 3 * HID, OFF_SAT = OFF_BC2 + 4, BLOB = OFF_SAT + 4;
+};
 
 // schedule emulation (render_fused.cu): budget[s] = total per-ray sample budget the reference host loop would grant
 int launch_schedule(const uint32_t* hist, uint32_t hist_bins, uint32_t num_scenes, uint32_t N, uint32_t max_steps,

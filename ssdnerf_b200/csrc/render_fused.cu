@@ -9,7 +9,7 @@
 //
 // This file holds variant P (shipped configs, 3x6 channels, hidden 64): fp32 planes, fp32 CUDA-core MLP
 // with weights broadcast from shared memory.  Variant S (3x32 channels, hidden 128) lives in
-// render_tc.cu (tcgen05 MMA, fp16 operands, fp32 accumulation in TMEM).
+// render_s2.cu (mma.sync, fp16 operands, fp32 accumulation).
 #include "common.cuh"
 #include <cstdlib>
 #include "render_common.cuh"
@@ -262,15 +262,15 @@ using namespace ssdnerf;
 extern "C" {
 
 size_t ssdnerf_decoder_blob_floats(int variant) {
-    if (variant == SSDNERF_DEC_P || variant == SSDNERF_DEC_P_SIMT || variant == SSDNERF_DEC_P_TC || variant == SSDNERF_DEC_P_MMA || variant == SSDNERF_DEC_P_MMA2) return DecP::BLOB;
-    if (variant == SSDNERF_DEC_S || variant == SSDNERF_DEC_S_MMA || variant == SSDNERF_DEC_S_TC) return ssdnerf::dec_s_blob_floats();
+    if (variant == SSDNERF_DEC_P || variant == SSDNERF_DEC_P_SIMT || variant == SSDNERF_DEC_P_MMA || variant == SSDNERF_DEC_P_MMA2) return DecP::BLOB;
+    if (variant == SSDNERF_DEC_S || variant == SSDNERF_DEC_S_MMA) return DecS::BLOB;
     return 0;
 }
 
 size_t ssdnerf_planes_bytes(int variant, uint32_t B, uint32_t Hp, uint32_t Wp) {
     const size_t texels = (size_t)B * 3 * Hp * Wp;
-    if (variant == SSDNERF_DEC_P || variant == SSDNERF_DEC_P_SIMT || variant == SSDNERF_DEC_P_TC || variant == SSDNERF_DEC_P_MMA || variant == SSDNERF_DEC_P_MMA2) return texels * 8 * sizeof(float);
-    if (variant == SSDNERF_DEC_S || variant == SSDNERF_DEC_S_MMA || variant == SSDNERF_DEC_S_TC) return texels * 32 * sizeof(__half);
+    if (variant == SSDNERF_DEC_P || variant == SSDNERF_DEC_P_SIMT || variant == SSDNERF_DEC_P_MMA || variant == SSDNERF_DEC_P_MMA2) return texels * 8 * sizeof(float);
+    if (variant == SSDNERF_DEC_S || variant == SSDNERF_DEC_S_MMA) return texels * 32 * sizeof(__half);
     return 0;
 }
 
@@ -278,12 +278,12 @@ int ssdnerf_pack_planes(int variant, const float* code, uint32_t B, uint32_t C, 
                         void* stream) {
     const size_t total = (size_t)B * 3 * Hp * Wp;
     if (total == 0) return 0;
-    if (((uintptr_t)planes & 31u) != 0) return set_error_msg(SSDNERF_ERR_ARG, "pack_planes: planes must be 32-byte aligned (256-bit texel loads)");
+    if (((uintptr_t)planes & 31u) != 0) return set_error_msg(SSDNERF_ERR_ARG, "pack_planes: planes must be 32-byte aligned (one texel = one 32-byte sector)");
     const uint32_t blocks = (uint32_t)((total + 255) / 256);
-    if (variant == SSDNERF_DEC_P || variant == SSDNERF_DEC_P_SIMT || variant == SSDNERF_DEC_P_TC || variant == SSDNERF_DEC_P_MMA || variant == SSDNERF_DEC_P_MMA2) {
+    if (variant == SSDNERF_DEC_P || variant == SSDNERF_DEC_P_SIMT || variant == SSDNERF_DEC_P_MMA || variant == SSDNERF_DEC_P_MMA2) {
         if (C != 6) return set_error_msg(SSDNERF_ERR_ARG, "pack_planes: variant P expects 6 channels per plane");
         k_pack_planes<float, 8><<<blocks, 256, 0, (cudaStream_t)stream>>>(code, B, C, Hp, Wp, (float*)planes);
-    } else if (variant == SSDNERF_DEC_S || variant == SSDNERF_DEC_S_MMA || variant == SSDNERF_DEC_S_TC) {
+    } else if (variant == SSDNERF_DEC_S || variant == SSDNERF_DEC_S_MMA) {
         if (C != 32) return set_error_msg(SSDNERF_ERR_ARG, "pack_planes: variant S expects 32 channels per plane");
         k_pack_planes<__half, 32><<<blocks, 256, 0, (cudaStream_t)stream>>>(code, B, C, Hp, Wp, (__half*)planes);
     } else {
@@ -350,7 +350,6 @@ int ssdnerf_render_fwd(const ssdnerf_render_args* a, void* stream_) {
     SSDNERF_CUDA_OK(cudaGetDevice(&dev));
     SSDNERF_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
 
-    if (a->variant == SSDNERF_DEC_P_TC) return ssdnerf::render_ptc_launch(p, a->emulate_schedule, hist, sms, stream);
     if (a->variant == SSDNERF_DEC_P_MMA) return ssdnerf::render_p2_launch(p, a->emulate_schedule, hist, sms, stream);
     if (a->variant == SSDNERF_DEC_P_MMA2 || a->variant == SSDNERF_DEC_P) return ssdnerf::render_p3_launch(p, a->emulate_schedule, hist, sms, stream);
     if (a->variant == SSDNERF_DEC_P_SIMT) {
@@ -379,7 +378,6 @@ int ssdnerf_render_fwd(const ssdnerf_render_args* a, void* stream_) {
         return 0;
     }
     if (a->variant == SSDNERF_DEC_S_MMA || a->variant == SSDNERF_DEC_S) return ssdnerf::render_s2_launch(p, a->emulate_schedule, hist, sms, stream);
-    if (a->variant == SSDNERF_DEC_S_TC) return ssdnerf::render_s_launch(p, a->emulate_schedule, hist, sms, stream);
     return set_error_msg(SSDNERF_ERR_ARG, "render_fwd: unknown decoder variant");
 }
 

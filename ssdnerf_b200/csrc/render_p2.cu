@@ -1,17 +1,13 @@
 // Fused inference renderer, variant P, warp-synchronous version (SSDNERF_DEC_P_MMA).
 //
-// Why a third P kernel: ncu of render_fused.cu (profiles/r01_ncu_render_p_simt.txt) shows 26 % of warp stalls are
-// instruction-fetch misses -- the fully unrolled 18x64 FMA block + 64-wide head loop is ~48 KB of SASS -- and the rest is spread
-// over FMA / LSU / MUFU issue; the CTA-synchronous tcgen05 kernel (render_ptc.cu) removes the FMAs but serialises gather, MMA and
-// heads inside a CTA (phase breakdown in profiles/r01_render_ptc_phase_breakdown.txt) and is latency-bound at 2 CTAs/SM.
-// Here every WARP is independent (no block barriers, no TMEM round trip):
+// Why a second P kernel: the fully unrolled 18x64 FMA block + 64-wide head loop of render_fused.cu is ~48 KB of SASS (instruction-fetch
+// misses) and its issue is spread over FMA / LSU / MUFU.  Here every WARP is independent (no block barriers):
 //   * lane = ray; features of the 32 samples of an iteration go to a per-warp shared-memory tile as split fp16 (hi, lo) rows;
 //   * the 18 -> 64 base layer (+bias through a constant-one column, K padded to 32) runs as warp-level tensor-core MMAs
 //     (mma.sync.m16n8k16 f16 x f16 -> f32, three split-precision products => fp32-class accuracy), 8 output columns at a time;
 //   * the heads are evaluated directly on the accumulator fragments inside a ROLLED loop over the 8 column tiles (small code),
 //     reduced over the 4 lanes of a quad with shuffles and handed back to the lane that owns the ray for compositing.
-// tcgen05 needs a CTA-wide M=128 tile and a TMEM round trip per sample batch; for a 32x64x32 product per warp the legacy
-// warp-level MMA is the better fit (DESIGN.md §3 discusses the trade-off with the measured numbers of all three kernels).
+// A warpgroup-wide wgmma needs a CTA-synchronous M=64 tile per sample batch; for a 32x64x32 product per warp the warp-level MMA fits.
 #include "common.cuh"
 #include "render_common.cuh"
 #include "dec_p.cuh"

@@ -1,8 +1,8 @@
 // Fused inference renderer, variant P, warp-synchronous version 2 (SSDNERF_DEC_P_MMA2; default for SSDNERF_DEC_P).
 //
 // Same structure as render_p2.cu (lane = ray for marching / gather / compositing, per-warp mma.sync base layer, heads evaluated on the
-// accumulator fragments) with the exponential work of the two hidden activations cut in half.  ncu of k_render_p3 (profiles/
-// r01_ncu_prof_render_P_MMA.txt): XU (MUFU) pipe 65 % busy, issue 60 %, 3 warps per scheduler -- 128 SiLU per sample at 1.5 MUFU each.
+// accumulator fragments) with the exponential work of the two hidden activations cut in half: the kernel is bound by the MUFU pipe
+// (128 SiLU per sample at 1.5 MUFU each).
 //   * density branch  s = silu(b),  colour branch  h = silu(b + f)  with  f = dir_net(SH16(d))  constant along a ray:
 //       exp(-(b + f)) = exp(-b) * exp(-f)   =>  ONE ex2 per hidden unit instead of two; exp(-f) is tabulated per (ray, unit) in shared
 //       memory when the ray tile starts (it takes the place of the f table of render_p2.cu, same footprint);
@@ -407,7 +407,7 @@ int render_p3_launch(const RenderParams& p, int emulate_schedule, uint32_t* hist
     static int mode = -1;
     if (mode < 0) {
         const char* e = getenv("SSDNERF_P3_MODE");
-        mode = 1;      // measured on B200 (dense / sphere workloads, G samples/s): noedf3 9.70 / 4.40, noedf4 9.48 / 4.55, edf3 9.20 / 4.20, k_render_p2 9.42 / 4.22
+        mode = 1;      // noedf3; the three modes have not been compared on the H100
         if (e) mode = !strcmp(e, "edf3") ? 0 : !strcmp(e, "noedf3") ? 1 : !strcmp(e, "noedf4") ? 2 : 1;
     }
     static int abl = -1;

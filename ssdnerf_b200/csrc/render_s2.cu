@@ -7,8 +7,6 @@
 //     activations never leave registers;
 //   * GEMM2 ([base_act | SH16] 144 -> 128 hidden + 1 density column) in a rolled loop over column tiles with the 128 -> 3 output
 //     layer applied to the accumulator fragments; quad shuffles reduce over columns and return sigma / rgb to the owning lane.
-// The CTA-synchronous tcgen05 kernel (render_tc.cu) issues 4x faster MMAs but pays two TMEM round trips and four block barriers
-// per sample batch with only 2 CTAs per SM resident; measured numbers for both are in profiles/ and DESIGN.md §3.
 #include "common.cuh"
 #include "render_common.cuh"
 #include "../../include/ssdnerf_b200.h"
@@ -19,7 +17,7 @@ constexpr int kS2Warps = 4, kS2Threads = kS2Warps * 32;
 constexpr int kS2ARow = 208;              // bytes per A1 row: 96 halves + 16 B pad (conflict-free ldmatrix)
 constexpr int kS2ShRow = 48;              // bytes per SH row: 16 halves + 16 B pad
 constexpr int kS2KF = 96, kS2Hid = 128, kS2K2 = 144;
-// blob offsets (render_tc.cu::DecS)
+// blob offsets (render_common.cuh::DecS)
 constexpr int kS2OffW1 = 0, kS2OffB1 = kS2Hid * kS2KF, kS2OffWd = kS2OffB1 + kS2Hid, kS2OffBd = kS2OffWd + kS2Hid,
               kS2OffWc0 = kS2OffBd + 4, kS2OffBc0 = kS2OffWc0 + kS2Hid * kS2K2, kS2OffWc2 = kS2OffBc0 + kS2Hid,
               kS2OffBc2 = kS2OffWc2 + 3 * kS2Hid, kS2OffSat = kS2OffBc2 + 4;

@@ -3,7 +3,7 @@
 // Guidance through the denoiser (lib/models/diffusions/gaussian_diffusion.py:193-216, `grad_through_unet=True`) and code
 // optimisation against the diffusion prior (lib/models/autodecoders/diffusion_nerf.py:313-404) differentiate the UNet with
 // FROZEN weights w.r.t. its input only, so the backward of every convolution / linear layer is a data-gradient GEMM -- the
-// same tcgen05 implicit-GEMM kernel as the forward (gemm_tc.cu / conv_row2.cu) run on transposed, tap-flipped weights -- and
+// same wgmma implicit-GEMM kernel as the forward (gemm_tc.cu / conv_row2.cu) run on transposed, tap-flipped weights -- and
 // what remains is here:
 //   GroupNorm(+scale/shift)(+SiLU) backward over a channel concat (two passes: group sums, then apply; the residual / shortcut
 //     gradient is added in the same pass and the result is split back into the two concatenated sources),
@@ -337,7 +337,7 @@ int ssdnerf_gn_bwd(const ssdnerf_gn_bwd_args* a, void* stream) {
     if (p.csum) SSDNERF_CUDA_OK(cudaMemsetAsync(p.csum, 0, (size_t)a->B * C * 2 * sizeof(float), s));
     const uint32_t cv = C / 8, threads = cv * (256 / cv);
     uint32_t chunks = (a->HW + 7) / 8;
-    const uint32_t max_chunks = (148 * 8 + a->B - 1) / a->B;
+    const uint32_t max_chunks = (device_sms() * 8 + a->B - 1) / a->B;
     if (chunks > max_chunks) chunks = max_chunks;
     p.pix_per_block = (a->HW + chunks - 1) / chunks;
     chunks = (a->HW + p.pix_per_block - 1) / p.pix_per_block;

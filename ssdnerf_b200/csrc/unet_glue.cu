@@ -330,7 +330,7 @@ int ssdnerf_gn_stats(const void* x1, uint32_t C1, const void* x2, uint32_t C2, u
     if (!B || !HW) return 0;
     // enough blocks to fill the machine, at least 64 pixels per block
     uint32_t chunks = (HW + 63) / 64;
-    const uint32_t max_chunks = (148 * 8 + B - 1) / B;
+    const uint32_t max_chunks = (device_sms() * 8 + B - 1) / B;
     if (chunks > max_chunks) chunks = max_chunks;
     const uint32_t ppb = (HW + chunks - 1) / chunks;
     chunks = (HW + ppb - 1) / ppb;
@@ -352,7 +352,7 @@ static int gn_apply_impl(const void* x1, uint32_t C1, const void* x2, uint32_t C
     if (groups > 64) return set_error_msg(SSDNERF_ERR_ARG, "gn_apply: at most 64 groups");
     const uint32_t threads = cv * (256 / cv);
     uint32_t chunks = (HW + 7) / 8;
-    const uint32_t max_chunks = (148 * 8 + B - 1) / B;
+    const uint32_t max_chunks = (device_sms() * 8 + B - 1) / B;
     if (chunks > max_chunks) chunks = max_chunks;
     const uint32_t ppb = (HW + chunks - 1) / chunks;
     chunks = (HW + ppb - 1) / ppb;

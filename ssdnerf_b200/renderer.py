@@ -11,12 +11,10 @@ from . import _lib as N
 DEC_P = 0   # shipped configs: base 18->64, density 64->1, dir_net 16->64, color 64->3
 DEC_S = 1   # TriPlaneDecoder class defaults: base 96->128, density 128->1, color 144->128->3
 DEC_P_SIMT = 2   # DEC_P on the CUDA cores (plain fp32)
-DEC_P_TC = 3     # DEC_P with a split-precision tcgen05 base layer
 DEC_P_MMA = 4    # DEC_P, warp-synchronous split-precision mma.sync base layer
 DEC_S_MMA = 5    # DEC_S, warp-synchronous mma.sync kernel
-DEC_S_TC = 6     # DEC_S, CTA-synchronous tcgen05 kernel
 DEC_P_MMA2 = 7   # DEC_P, warp-synchronous v2 (shared exponentials, tensor-core dir_net): what DEC_P selects
-_VARIANT_C = {DEC_P: 6, DEC_S: 32, DEC_P_SIMT: 6, DEC_P_TC: 6, DEC_P_MMA: 6, DEC_S_MMA: 32, DEC_S_TC: 32, DEC_P_MMA2: 6}
+_VARIANT_C = {DEC_P: 6, DEC_S: 32, DEC_P_SIMT: 6, DEC_P_MMA: 6, DEC_S_MMA: 32, DEC_P_MMA2: 6}
 
 
 def detect_variant(params):
@@ -40,7 +38,7 @@ def _plane_major(w, C):
 
 def pack_decoder_blob(params, variant=None, sigmoid_saturation=0.001, device='cuda'):
     """Flatten decoder weights into the fp32 blob the kernels read (layout documented in csrc/render_fused.cu
-    `DecP` and csrc/render_tc.cu `DecS`)."""
+    `DecP` and csrc/render_common.cuh `DecS`)."""
     if variant is None:
         variant = detect_variant(params)
     p = {k: v.detach().float() for k, v in params.items()}       # packed where the weights live: no host round trip per optimiser step
@@ -49,13 +47,13 @@ def pack_decoder_blob(params, variant=None, sigmoid_saturation=0.001, device='cu
     def pad(t, n):
         return torch.cat([t, torch.zeros(n, device=src)])
     tail = torch.tensor([sigmoid_saturation, 0, 0, 0], dtype=torch.float32, device=src)
-    if variant in (DEC_P, DEC_P_SIMT, DEC_P_TC, DEC_P_MMA, DEC_P_MMA2):
+    if variant in (DEC_P, DEC_P_SIMT, DEC_P_MMA, DEC_P_MMA2):
         w1 = _plane_major(p['base_net.0.weight'], 6).t().contiguous()           # [18][64], row k = plane*6+c
         parts = [w1.reshape(-1), p['base_net.0.bias'],
                  p['density_net.0.weight'].reshape(-1), pad(p['density_net.0.bias'], 3),
                  p['dir_net.0.weight'].t().contiguous().reshape(-1), p['dir_net.0.bias'],      # [16][64]
                  p['color_net.0.weight'].reshape(-1), pad(p['color_net.0.bias'], 1), tail]
-    elif variant in (DEC_S, DEC_S_MMA, DEC_S_TC):
+    elif variant in (DEC_S, DEC_S_MMA):
         w1 = _plane_major(p['base_net.0.weight'], 32)                             # [128][96] (N x K, K contiguous)
         wc0 = p['color_net.0.weight']                                             # [128][144]: cols 0..127 base_act, 128..143 SH
         parts = [w1.reshape(-1), p['base_net.0.bias'],

@@ -1,10 +1,10 @@
-"""`DenoisingUnetMod` -- the reference's 2-D UNet over triplane latents, executed by hand-written sm_100a kernels.
+"""`DenoisingUnetMod` -- the reference's 2-D UNet over triplane latents, executed by hand-written sm_90a kernels.
 
 Plugin surface kept from the reference (lib/models/architecture/ddpm/denoising.py:12-216, modules.py:12-129):
 constructor kwargs, `forward(x_t, t, label=None, concat_cond=None)` and the state-dict key layout (SURVEY.md
 Appendix D) so released checkpoints load unchanged.  The nn.Module tree below only HOLDS parameters; compute goes
 through `UNetEngine`, which packs the weights to fp16 once and issues the C-ABI kernels of include/ssdnerf_b200.h §4:
-implicit-GEMM 3x3 / 1x1 convolutions and attention GEMMs on tcgen05 tensor cores, GroupNorm(+scale/shift)+SiLU,
+implicit-GEMM 3x3 / 1x1 convolutions and attention GEMMs on wgmma tensor cores, GroupNorm(+scale/shift)+SiLU,
 softmax and layout glue as fused memory-bound kernels.  Forward semantics of the blocks the reference inherits from
 mmgen 0.7.2 are restated per SURVEY.md Appendix B.  Inference only (no autograd through the engine).
 """
@@ -262,8 +262,8 @@ class UNetEngine:
                 f'native UNet engine: channel widths must be multiples of 64 with GroupNorm(32) (every paper config: base 128); got widths '
                 f'{widths}, {m.num_groups} groups (configs/new_cfgs/*_tiled.py builds and loads checkpoints but has no kernels yet)')
         self.flash_attention = True      # False: unfused scores -> softmax -> PV composition (A/B tests)
-        # 128x128-level resblocks: GroupNorm + SiLU inside the conv kernel (csrc/conv_row2_gn.cu).  Opt-in: measured 98 us per 128->128 layer
-        # against 22 + 59 us for the GroupNorm-apply pass + CTA-pair row-pair convolution (profiles/r01_gemm_pipeline_prof.txt)
+        # 128x128-level resblocks: GroupNorm + SiLU inside the row-pair conv kernel (csrc/conv_row2.cu).  Opt-in (SSDNERF_FUSED_GN_CONV=1):
+        # the default is the GroupNorm-apply pass followed by the row-pair convolution
         self.fused_gn_conv = os.environ.get('SSDNERF_FUSED_GN_CONV', '0') == '1'
         self.H, self.W = m.image_size
         self.bufs = {}

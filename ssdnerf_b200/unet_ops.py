@@ -28,7 +28,7 @@ class GemmArgs(ctypes.Structure):
     ]
 
 
-GEMM_PROF = None    # set to a uint64[8] CUDA tensor to collect per-role pipeline wait cycles (debug)
+GEMM_PROF = None    # set to a uint64[8] CUDA tensor to collect the generic GEMM kernel's pipeline wait cycles (debug, ssdnerf_gemm_args.debug_cycles)
 GEMM_LOG = None     # set to a list to record (M, N, K, taps, bn, cluster, batched, fused_stats) of every launch (profiling scripts)
 
 
@@ -284,7 +284,7 @@ class ConvGnArgs(ctypes.Structure):
         ('x1', N.c_void_p), ('C1', N.c_u32), ('x2', N.c_void_p), ('C2', N.c_u32), ('B', N.c_u32), ('H', N.c_u32),
         ('q1', N.c_void_p), ('q2', N.c_void_p), ('gamma', N.c_void_p), ('beta', N.c_void_p), ('scale_shift', N.c_void_p),
         ('ss_batch_stride', c_ll), ('eps', N.c_f32), ('w', N.c_void_p), ('w_rows', N.c_u32), ('bias', N.c_void_p),
-        ('residual', N.c_void_p), ('out', N.c_void_p), ('qstats', N.c_void_p), ('coef_workspace', N.c_void_p), ('debug_cycles', N.c_void_p),
+        ('residual', N.c_void_p), ('out', N.c_void_p), ('qstats', N.c_void_p), ('coef_workspace', N.c_void_p),
     ]
 
 
@@ -314,8 +314,6 @@ def conv3x3_gn_f16(x1, q1, gamma, beta, wp, bias=None, x2=None, q2=None, scale_s
     if coef_ws is None:
         coef_ws = torch.empty(B * (C1 + (x2.shape[-1] if x2 is not None else 0)) * 2, dtype=torch.float32, device=x1.device)
     a.coef_workspace = coef_ws.data_ptr()
-    if GEMM_PROF is not None:
-        a.debug_cycles = GEMM_PROF.data_ptr()
     if GEMM_LOG is not None:
         GEMM_LOG.append(dict(M=B * H * W, N=128, K=int(a.C1) + int(a.C2), taps=9, bn=128, cluster=1, batched=0, qstats=bool(a.qstats), f32=0, fused_gn=True))
     N.check(N.lib().ssdnerf_conv3x3_gn_f16(ctypes.byref(a), N.stream_ptr()))

@@ -1,4 +1,7 @@
-"""tcgen05 GEMM / implicit-GEMM conv (C-ABI ssdnerf_gemm_f16) vs PyTorch fp32 on the same fp16-rounded operands."""
+"""wgmma GEMM / implicit-GEMM conv (C-ABI ssdnerf_gemm_f16) vs PyTorch fp32 on the same fp16-rounded operands.
+
+Some shapes have more than twice as many output tiles as an H100 has SMs, so the persistent kernels carry their pipelines
+(stage phases, staged rows, weight tiles, statistics flushes) across several tiles per CTA."""
 import pytest
 import torch
 
@@ -10,7 +13,7 @@ def _check(out, ref, tol=2e-3):
     assert err < tol, f'rel err {err}'
 
 
-@pytest.mark.parametrize('M,N,K,bn', [(256, 128, 64, 128), (1000, 320, 192, 0), (128, 64, 128, 64), (4096, 512, 1024, 256)])
+@pytest.mark.parametrize('M,N,K,bn', [(256, 128, 64, 128), (1000, 320, 192, 0), (128, 64, 128, 64), (4096, 512, 1024, 256), (8960, 512, 256, 128)])
 def test_plain_gemm(cuda, M, N, K, bn):
     from ssdnerf_b200 import unet_ops as U
     g = torch.Generator().manual_seed(M + N + K)
@@ -68,18 +71,22 @@ def test_batched_attention_gemms(cuda):
 
 
 @pytest.mark.parametrize('cluster', [1, 2, 4, 8])
-@pytest.mark.parametrize('B,H,W,Cin,Cout,bn', [(3, 64, 64, 128, 256, 256), (2, 128, 128, 64, 128, 128), (5, 8, 8, 512, 512, 256), (1, 32, 32, 256, 256, 128)])
+@pytest.mark.parametrize('B,H,W,Cin,Cout,bn', [(3, 64, 64, 128, 256, 256), (2, 128, 128, 64, 128, 128), (5, 8, 8, 512, 512, 256), (1, 32, 32, 256, 256, 128),
+                                              (5, 64, 64, 128, 256, 128)])
 def test_conv3x3_cluster_multicast(cuda, cluster, B, H, W, Cin, Cout, bn):
-    """CTA pairs along M with TMA multicast of the weight tile (odd tile counts exercise the zero-filled tail CTA)"""
+    """clusters along M with TMA multicast of the weight tile (odd tile counts exercise the zero-filled tail CTA), fused quad statistics"""
     from ssdnerf_b200 import unet_ops as U
     g = torch.Generator().manual_seed(B * H + Cin + cluster)
     x = torch.randn(B, H, W, Cin, generator=g).half().to(cuda)
     w = torch.randn(Cout, Cin, 3, 3, generator=g) * 0.05
     b = torch.randn(Cout, generator=g).to(cuda)
     res = torch.randn(B, H, W, Cout, generator=g).half().to(cuda)
-    out = U.conv3x3_f16(x, U.pack_conv_weight(w).to(cuda), Cout, bias=b, residual=res, bn=bn, cluster=cluster)
+    q = torch.zeros(B, Cout // 4, 2, device=cuda)
+    out = U.conv3x3_f16(x, U.pack_conv_weight(w).to(cuda), Cout, bias=b, residual=res, bn=bn, cluster=cluster, qstats=q)
     ref = torch.nn.functional.conv2d(x.float().permute(0, 3, 1, 2), w.half().float().to(cuda), b, padding=1).permute(0, 2, 3, 1) + res.float()
     _check(out, ref)
+    rq = ref.reshape(B, -1, Cout // 4, 4)
+    torch.testing.assert_close(q, torch.stack([rq.sum(dim=(1, 3)), (rq * rq).sum(dim=(1, 3))], dim=-1), rtol=2e-3, atol=2e-2)
 
 
 def test_plain_gemm_cluster(cuda):
@@ -92,7 +99,7 @@ def test_plain_gemm_cluster(cuda):
     _check(out, a.float() @ w.float().t())
 
 
-@pytest.mark.parametrize('B,H,C1,C2', [(2, 8, 128, 0), (1, 128, 64, 0), (3, 6, 128, 128), (2, 4, 256, 128)])
+@pytest.mark.parametrize('B,H,C1,C2', [(2, 8, 128, 0), (1, 128, 64, 0), (3, 6, 128, 128), (2, 4, 256, 128), (5, 128, 64, 64)])
 def test_conv3x3_row_pair_kernel(cuda, B, H, C1, C2):
     """128-pixel-wide rows, 128 output channels: row-pair kernel with halo reuse (algo 2) == generic tile kernel (algo 1) == fp32 conv,
     including image borders, the skip-concat second input, bias, residual and the fused quad statistics"""
@@ -118,7 +125,8 @@ def test_conv3x3_row_pair_kernel(cuda, B, H, C1, C2):
     torch.testing.assert_close(stats[2], stats[1], rtol=1e-3, atol=5e-2)
 
 
-@pytest.mark.parametrize('B,H,C1,C2,use_ss', [(2, 8, 128, 0, False), (1, 128, 128, 0, True), (3, 6, 128, 128, False), (2, 4, 256, 128, True)])
+@pytest.mark.parametrize('B,H,C1,C2,use_ss', [(2, 8, 128, 0, False), (1, 128, 128, 0, True), (3, 6, 128, 128, False), (2, 4, 256, 128, True),
+                                              (5, 128, 128, 128, True)])
 def test_fused_groupnorm_silu_conv(cuda, B, H, C1, C2, use_ss):
     """GroupNorm(32) (+ scale/shift) + SiLU + conv3x3 on RAW inputs in one kernel vs the gn_apply pass followed by the convolution kernels
     and vs fp32 PyTorch GroupNorm -> SiLU -> conv2d.  The fused kernel evaluates SiLU on packed halves (tanh.approx.f16x2): its normalised

@@ -14,7 +14,7 @@ pytestmark = pytest.mark.gpu
 # fp32 CUDA-core MLP (variant P): only round-off / fast-intrinsic differences vs the fp32 oracle
 TOL_P = dict(rtol=2e-4, atol=2e-5)
 # fp16 tensor-core MLP + fp16 planes (variant S): BASELINE.json north_star "1e-3 relative fp16 tolerance" on rendered RGB, taken on the
-# image range [0, 1].  Measured on the B200: max abs error 8.7e-5 (dense grid) / 5.1e-5 (sphere); the bar is half the stated tolerance.
+# image range [0, 1]; the bar is half the stated tolerance.
 TOL_S = dict(rtol=0, atol=5e-4)
 
 
@@ -41,12 +41,12 @@ def _run_gpu(variant, vid, params, code, bf, poses, intr, res, cuda, max_steps, 
     return {k: (v.cpu().numpy() if v is not None else None) for k, v in out.items()}
 
 
-@pytest.mark.parametrize('variant', ['P', 'P_SIMT', 'P_TC', 'P_MMA', 'P_MMA2', 'S', 'S_TC'])
+@pytest.mark.parametrize('variant', ['P', 'P_SIMT', 'P_MMA', 'P_MMA2', 'S'])
 @pytest.mark.parametrize('grid', ['ones', 'sphere'])
 def test_config1_explicit_rays(cuda, variant, grid):
     """SURVEY §8d config 1: 64x64 render, max_steps=32 (fixed step dt_max), bit-exact integer trace."""
     from ssdnerf_b200 import renderer as R
-    vid = {'P': R.DEC_P, 'P_SIMT': R.DEC_P_SIMT, 'P_TC': R.DEC_P_TC, 'P_MMA': R.DEC_P_MMA, 'P_MMA2': R.DEC_P_MMA2, 'S': R.DEC_S, 'S_TC': R.DEC_S_TC}[variant]
+    vid = {'P': R.DEC_P, 'P_SIMT': R.DEC_P_SIMT, 'P_MMA': R.DEC_P_MMA, 'P_MMA2': R.DEC_P_MMA2, 'S': R.DEC_S}[variant]
     code, poses, intr = config1(variant[0])
     params = rp.make_decoder_params(variant[0], 0)
     bf = _bitfields()[grid]

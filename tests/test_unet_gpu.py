@@ -1,13 +1,13 @@
-"""UNet / DDIM on the GPU (tcgen05 GEMMs, fp16 operands + activation storage, fp32 accumulation) vs the fp32 oracle
+"""UNet / DDIM on the GPU (wgmma GEMMs, fp16 operands + activation storage, fp32 accumulation) vs the fp32 oracle
 (oracle/unet_port.py, pinned to the reference's own code by tests/test_reference_pin_cpu.py).
 
 Tolerance.  BASELINE.json north_star: "denoised triplanes within 1e-3 relative fp16 tolerance".  An fp32 oracle cannot be matched to
-1e-3 by ANY single-pass 10/11-bit-mantissa tensor-core path: tests/perf/precision_probe.py (profiles/r02_precision_probe.txt) injects
+1e-3 by ANY single-pass 10/11-bit-mantissa tensor-core path: tests/perf/precision_probe.py injects
 the roundings one at a time into the fp32 oracle at full size -- fp16 GEMM operands alone 1.28e-3, the reference's own default
 (cuDNN TF32 convolutions, SURVEY.md Appendix C) 1.28e-3, fp16 storage of h1 +0.62e-3, of the residual stream +0.67e-3 (RSS total
-1.54e-3 = what the GPU measures).  The bars below are therefore stated against that floor: one evaluation <= 2.0e-3 relative L2
-(measured 1.4-1.5e-3), i.e. within 1.2x of the reference's own TF32 deviation from fp32.  The quantity north_star actually names -- the
-DENOISED TRIPLANE, i.e. the output of the whole 50-step chain -- is within 1e-3: measured 4.5e-4 at full size (the sampler is contractive,
+1.54e-3).  The bars below are therefore stated against that floor: one evaluation <= 2.0e-3 relative L2,
+i.e. within 1.2x of the reference's own TF32 deviation from fp32.  The quantity north_star actually names -- the
+DENOISED TRIPLANE, i.e. the output of the whole 50-step chain -- is within 1e-3 at full size (the sampler is contractive,
 per-evaluation noise does not accumulate), asserted below."""
 import math
 
@@ -123,7 +123,7 @@ def test_ddim_graph_equals_eager_and_tracks_oracle(cuda):
     ref = up.ddim_sample(lambda x, t: up.unet_forward(sd, spec, x, t), noise, dv, num_timesteps=8)
     err = _rel_l2(a, ref)
     print('ddim 8 steps rel l2', err)
-    assert err < 1e-3          # north_star: denoised triplanes within 1e-3 relative; measured 4.5e-4 on the B200
+    assert err < 1e-3          # north_star: denoised triplanes within 1e-3 relative
     # schedule tables equal the oracle's float64 restatement
     np.testing.assert_array_equal(diff.alphas_bar, dv['alphas_bar'])
     assert torch.equal(diff.ddim_timesteps(50), up.ddim_timesteps(1000, 50))
@@ -173,7 +173,7 @@ def test_full_size_50_step_ddim_vs_fp32_oracle(cuda):
         ref = up.ddim_sample(lambda x, t: up.unet_forward(sdg, spec, x, t.to(x.device)), noise.to(cuda), dv, num_timesteps=50, clip_range=(-2, 2)).cpu()
     err = _rel_l2(out, ref)
     print('full-size 50-step DDIM rel l2', err, 'max abs', float((out - ref).abs().max()), 'ref rms', float(ref.pow(2).mean().sqrt()))
-    assert err < 1e-3          # north_star: denoised triplanes within 1e-3 relative; measured 4.5e-4 on the B200
+    assert err < 1e-3          # north_star: denoised triplanes within 1e-3 relative
 
 
 def test_fused_quad_stats_match_tensor(cuda):
