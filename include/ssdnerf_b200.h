@@ -92,18 +92,15 @@ SSDNERF_API int ssdnerf_sh_encode_backward(const float* grad, const float* input
  *      lib/models/autodecoders/base_nerf.py:520-523        (image + bg * (1 - weights_sum), optional)
  * ---------------------------------------------------------------------------------------------- */
 
-/* Decoder variants (template instantiations). */
+/* Decoder variants; every entry point taking a variant returns SSDNERF_ERR_ARG (size queries: 0) for any other value. */
 #define SSDNERF_DEC_P 0 /* shipped configs: base 3*6->64, density 64->1, dir_net 16->64, color 64->3
-                           (configs/paper_cfgs/ssdnerf_cars_uncond.py:40-51) */
-#define SSDNERF_DEC_P_SIMT 2 /* decoder P on the CUDA cores in plain fp32 (csrc/render_fused.cu) */
-#define SSDNERF_DEC_P_MMA 4  /* decoder P, warp-synchronous: per-warp split-precision mma.sync base layer (csrc/render_p2.cu) */
-#define SSDNERF_DEC_P_MMA2 7 /* decoder P, warp-synchronous v2: one exponential per hidden unit shared by both branches, dir_net on the
-                                tensor cores, one reciprocal per four sigmoids (csrc/render_p3.cu); what SSDNERF_DEC_P selects */
-#define SSDNERF_DEC_S_MMA 5  /* decoder S, warp-synchronous mma.sync kernel (csrc/render_s2.cu); what SSDNERF_DEC_S selects */
+                           (configs/paper_cfgs/ssdnerf_cars_uncond.py:40-51); fp32 planes, warp-synchronous kernel with the base layer
+                           and dir_net as split-precision mma.sync, fp32 accumulation (csrc/render_p3.cu) */
 #define SSDNERF_DEC_S 1 /* TriPlaneDecoder class defaults: base 3*32->128, density 128->1, color (128+16)->128->3
-                           (lib/models/decoders/triplane_decoder.py:24-39) */
+                           (lib/models/decoders/triplane_decoder.py:24-39); fp16 planes, warp-synchronous kernel with both hidden
+                           layers as fp16 mma.sync, fp32 accumulation (csrc/render_s2.cu) */
 
-/* Size in floats of the packed fp32 decoder-weight blob for a variant (layout: ssdnerf_b200/decoder_pack.py). */
+/* Size in floats of the packed fp32 decoder-weight blob for a variant (layout: ssdnerf_b200/renderer.py pack_decoder_blob). */
 SSDNERF_API size_t ssdnerf_decoder_blob_floats(int variant);
 
 /* Re-layout one batch of triplanes for the gather:
@@ -150,7 +147,6 @@ typedef struct ssdnerf_render_args {
     int32_t* num_samples;     /* samples composited per ray, optional */
     int32_t* voxel_trace;     /* optional [B][N][trace_cap] occupancy-bit index of every composited sample (-1 padded) */
     uint32_t trace_cap;
-    void* debug_phase_cycles; /* optional uint64[8]: per-phase clock64 totals of thread 0 of every CTA (SSDNERF_DEC_P / SSDNERF_DEC_P_MMA2: decode iterations, active lanes) */
     /* --- scratch */
     void* workspace;          /* >= ssdnerf_render_workspace_bytes(...) bytes, 16-byte aligned */
     size_t workspace_bytes;

@@ -1,6 +1,6 @@
 """ssdnerf_b200 -- H100-native (sm_90a) implementation of SSDNeRF's two data-parallel hot paths.
 
-    renderer / decoders : fused occupancy-grid triplane renderer  (csrc/render_fused.cu, csrc/render_p3.cu, csrc/render_s2.cu)
+    renderer / decoders : fused occupancy-grid triplane renderer  (csrc/render.cu, csrc/render_p3.cu, csrc/render_s2.cu)
     density             : occupancy-grid builder                   (csrc/density.cu)
     unet / diffusion    : DDIM loop over triplane latents          (csrc/gemm_tc.cu, csrc/unet_glue.cu)
     raymarching / shencoder / activation : one-to-one mirrors of the reference's lib.ops (csrc/legacy_ops.cu)

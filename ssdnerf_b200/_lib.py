@@ -37,7 +37,6 @@ class RenderArgs(ctypes.Structure):
         ('max_steps', c_u32), ('emulate_schedule', c_int),
         ('weights_sum', c_void_p), ('depth', c_void_p), ('image', c_void_p), ('rgb_blend', c_void_p),
         ('num_samples', c_void_p), ('voxel_trace', c_void_p), ('trace_cap', c_u32),
-        ('debug_phase_cycles', c_void_p),
         ('workspace', c_void_p), ('workspace_bytes', c_size_t),
     ]
 

@@ -1,12 +1,12 @@
-// Variant P decoder pieces shared by the fused renderer (render_fused.cu) and the occupancy-grid builder (density.cu).
+// Variant P decoder pieces shared by the fused renderers (render_p3.cu, render_train.cu), the stand-alone point decode
+// (point_decode.cu) and the occupancy-grid builder (density.cu).
 #pragma once
 #include "common.cuh"
 
 namespace ssdnerf {
 
 // ------------------------------------------------------------------------------------------------
-// Variant P decoder: weights in shared memory, one sample per lane.
-// blob layout (floats), see ssdnerf_b200/decoder_pack.py:
+// Variant P decoder blob layout (floats), written by renderer.pack_decoder_blob:
 //   W1[18][64] (row k = plane*6 + c) | b1[64] | Wd[64] | bd,0,0,0 | Wdir[16][64] | bdir[64] | Wc[3][64] | bc[3],0 | sat,0,0,0
 // ------------------------------------------------------------------------------------------------
 struct DecP {
@@ -18,11 +18,6 @@ struct DecP {
 
 constexpr int kWarpsPerCta = 4;
 constexpr int kCtaThreads = kWarpsPerCta * 32;
-
-struct BitfieldLoader {
-    const uint8_t* __restrict__ g;
-    __device__ __forceinline__ uint32_t operator()(uint32_t byte) const { return __ldg(g + byte); }
-};
 
 // one 32-byte texel (8 floats, 6 used) as a 128-bit + a 64-bit read-only load of the same 32-byte sector (the widest loads sm_90 has)
 struct Texel8 { float4 lo; float2 hi; };

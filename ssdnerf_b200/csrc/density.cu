@@ -299,8 +299,8 @@ int ssdnerf_density_update(int variant, const void* planes, uint32_t plane_h, ui
                            uint32_t num_scenes, uint32_t grid_size, float bound, const float* jitter, float decay,
                            void* density_grid, int grid_is_half, void* workspace, void* stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
-    const bool is_s = variant == SSDNERF_DEC_S || variant == SSDNERF_DEC_S_MMA;
-    if (!is_s && variant != SSDNERF_DEC_P && variant != SSDNERF_DEC_P_SIMT && variant != SSDNERF_DEC_P_MMA && variant != SSDNERF_DEC_P_MMA2)
+    const bool is_s = variant == SSDNERF_DEC_S;
+    if (!is_s && variant != SSDNERF_DEC_P)
         return set_error_msg(SSDNERF_ERR_ARG, "density_update: unknown decoder variant");
     if (!planes || !decoder_blob || !density_grid || !workspace) return set_error_msg(SSDNERF_ERR_ARG, "density_update: NULL argument");
     if (grid_size == 0 || grid_size > 1024 || (grid_size & (grid_size - 1))) return set_error_msg(SSDNERF_ERR_ARG, "density_update: grid_size must be a power of two");

@@ -97,7 +97,7 @@ extern "C" int ssdnerf_point_decode(int variant, const void* planes, uint32_t pl
                                     const float* xyzs, const float* dirs, const long long* scene_offsets, uint32_t num_scenes,
                                     unsigned long long num_points, float* sigmas, float* rgbs, void* stream) {
     using namespace ssdnerf;
-    if (variant != SSDNERF_DEC_P && variant != SSDNERF_DEC_P_SIMT && variant != SSDNERF_DEC_P_MMA && variant != SSDNERF_DEC_P_MMA2)
+    if (variant != SSDNERF_DEC_P)
         return set_error_msg(SSDNERF_ERR_ARG, "ssdnerf_point_decode: only the shipped-config decoder (variant P) has a stand-alone point decode");
     if (!planes || !decoder_blob || !xyzs || !scene_offsets || !sigmas) return set_error_msg(SSDNERF_ERR_ARG, "ssdnerf_point_decode: NULL argument");
     if (rgbs && !dirs) return set_error_msg(SSDNERF_ERR_ARG, "ssdnerf_point_decode: rgbs requested without dirs");

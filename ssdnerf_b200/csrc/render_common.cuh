@@ -1,5 +1,5 @@
-// Parameters and ray set-up shared by the fused render kernels (variant P: render_fused.cu / render_p2.cu / render_p3.cu,
-// variant S: render_s2.cu).
+// Parameters, ray set-up and warp-level mma.sync helpers shared by the fused render kernels (variant P: render_p3.cu,
+// variant S: render_s2.cu; entry points and the schedule emulation: render.cu).
 #pragma once
 #include "common.cuh"
 
@@ -24,7 +24,6 @@ struct RenderParams {
     uint32_t* hist; uint32_t hist_bins;
     uint32_t* budget;          // [B] emulated per-ray sample budget
     uint32_t hard_cap, max_steps;
-    unsigned long long* prof;  // optional [8] phase cycle counters (debug instrumentation; NULL in production)
     int patch_tiles;           // camera mode: a 32-ray tile is an 8x4 pixel patch instead of 32 consecutive pixels
 };
 
@@ -62,10 +61,32 @@ __device__ __forceinline__ void make_ray(const RenderParams& p, uint32_t scene, 
     r.rdx = __fdiv_rn(1.0f, r.dx); r.rdy = __fdiv_rn(1.0f, r.dy); r.rdz = __fdiv_rn(1.0f, r.dz);
 }
 
-// variant P, warp-level mma.sync (render_p2.cu)
-int render_p2_launch(const RenderParams& p, int emulate_schedule, uint32_t* hist, int sms, cudaStream_t stream);
+// occupancy bitfield of one scene, read through the read-only cache (the GridLoader of `probe`)
+struct BitfieldLoader {
+    const uint8_t* __restrict__ g;
+    __device__ __forceinline__ uint32_t operator()(uint32_t byte) const { return __ldg(g + byte); }
+};
 
-// variant P, warp-level mma.sync, shared exponentials + tensor-core dir_net (render_p3.cu)
+// (x0, x1) -> packed fp16 hi = fp16(x), lo = fp16(x - hi): two fp16 products recover fp32-class accuracy (packed F2FP converts)
+__device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_t& lo) {
+    const __half2 h = __floats2half2_rn(x0, x1);
+    const float2 hf = __half22float2(h);
+    const __half2 l = __floats2half2_rn(x0 - hf.x, x1 - hf.y);
+    hi = *reinterpret_cast<const uint32_t*>(&h);
+    lo = *reinterpret_cast<const uint32_t*>(&l);
+}
+// four 8x8 b16 matrices from shared memory: lane l supplies the row address of matrix l / 8
+__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t* r) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
+}
+// d (16 x 8 fp32) += a (16 x 16 fp16, row) * b (16 x 8 fp16, col)
+__device__ __forceinline__ void mma_16816(float* d, const uint32_t* a, uint2 b) {
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b.x), "r"(b.y));
+}
+
+// variant P, split-precision mma.sync base layer and dir_net (render_p3.cu)
 int render_p3_launch(const RenderParams& p, int emulate_schedule, uint32_t* hist, int sms, cudaStream_t stream);
 
 // variant S, warp-level mma.sync (render_s2.cu)
@@ -79,7 +100,7 @@ struct DecS {
                          OFF_BC2 = OFF_WC2 + 3 * HID, OFF_SAT = OFF_BC2 + 4, BLOB = OFF_SAT + 4;
 };
 
-// schedule emulation (render_fused.cu): budget[s] = total per-ray sample budget the reference host loop would grant
+// schedule emulation (render.cu): budget[s] = total per-ray sample budget the reference host loop would grant
 int launch_schedule(const uint32_t* hist, uint32_t hist_bins, uint32_t num_scenes, uint32_t N, uint32_t max_steps,
                     uint32_t* budget, cudaStream_t stream);
 

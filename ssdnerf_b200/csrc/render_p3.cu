@@ -1,33 +1,26 @@
-// Fused inference renderer, variant P, warp-synchronous version 2 (SSDNERF_DEC_P_MMA2; default for SSDNERF_DEC_P).
+// Fused inference renderer, variant P (shipped configs: 3x6 channels, hidden 64): the kernel behind SSDNERF_DEC_P.
 //
-// Same structure as render_p2.cu (lane = ray for marching / gather / compositing, per-warp mma.sync base layer, heads evaluated on the
-// accumulator fragments) with the exponential work of the two hidden activations cut in half: the kernel is bound by the MUFU pipe
-// (128 SiLU per sample at 1.5 MUFU each).
-//   * density branch  s = silu(b),  colour branch  h = silu(b + f)  with  f = dir_net(SH16(d))  constant along a ray:
-//       exp(-(b + f)) = exp(-b) * exp(-f)   =>  ONE ex2 per hidden unit instead of two; exp(-f) is tabulated per (ray, unit) in shared
-//       memory when the ray tile starts (it takes the place of the f table of render_p2.cu, same footprint);
-//   * b + f itself comes out of the tensor cores: the 16 -> 64 dir_net is a K = 16 mma.sync on SH fragments held in registers for the
-//       whole tile (split precision like the base layer, bias folded into the constant SH basis 0), accumulated on top of the base-layer
-//       accumulator -- no per-sample loads or adds for f, and the 1024-FMA per-ray SIMT evaluation of dir_net is gone;
-//   * one reciprocal serves FOUR sigmoids (two units x two branches): r = 1 / (d1 d2 d3 d4), every 1/d_i recovered with multiplies
-//       (exponents clamped to 2^30 so the product stays finite) => 3 MUFU per 4 SiLU instead of 6;
-//   * the -log2(e) scale of the exponent is folded into the staged weights (the MMA delivers z = -log2(e) * b) and undone in the head
-//       weights, which removes the scaling multiplies from the inner loop.
-// Arithmetic stays fp32-class (split-precision products, fp32 accumulation): same parity bars as render_p2.cu.
+// Every warp owns a tile of 32 rays and nothing is synchronised across warps. A lane marches its own ray through the occupancy grid,
+// gathers the 18 bilinear triplane features of its next sample and composites; the MLP runs on the tensor cores for the whole warp.
+//   * base layer 18 -> 64 as split-precision mma.sync: features and weights are each split into fp16 hi + lo halves and the three
+//     significant products (lo*hi, hi*lo, hi*hi) accumulate in fp32, which keeps fp32-class accuracy; the bias rides on a constant-one
+//     column of the A tile;
+//   * dir_net 16 -> 64 on the tensor cores on top of the base accumulator: the SH16 fragments of the ray direction stay in registers for
+//     the whole tile (bias folded into the constant SH basis 0), so the colour branch's pre-activation b + f comes out of the MMA;
+//   * -log2(e) is folded into the staged weights (the MMA delivers z = -log2(e) * pre-activation, the argument of ex2) and -ln 2 into the
+//     head weights, which takes the scaling multiplies out of the inner loop;
+//   * the density and colour heads are evaluated on the accumulator fragments: SiLU in pairs, two ex2 and one rcp per pair
+//     (one reciprocal of the product of the two denominators), then quad shuffles reduce over the columns.
 #include "common.cuh"
 #include "render_common.cuh"
 #include "dec_p.cuh"
 #include "../../include/ssdnerf_b200.h"
-#include <cstddef>
-#include <cstdlib>
-#include <cstring>
 
 namespace ssdnerf {
 
 constexpr float kLog2e = 1.4426950408889634f, kLn2 = 0.6931471805599453f;
 constexpr int kP3Warps = 4, kP3Threads = kP3Warps * 32;
 constexpr int kARow3 = 80;                // bytes per A-tile row: 32 halves + 16 B pad (conflict-free ldmatrix / 16-byte stores)
-constexpr int kEdfStride = 72;           // floats per dirf row: 64 + 8 pad (2-wavefront 8-byte fragment loads)
 constexpr int kOneK3 = 24;                // K index of the constant-one (bias) column
 
 struct SmemP3 {
@@ -37,34 +30,16 @@ struct SmemP3 {
     alignas(16) uint4 dfrag[8][32];                            // dir_net: [n-tile][lane] = {b0,b1 hi, b0,b1 lo}, K = 16 SH values
     float4 heads[DecP::HID];                                   // {wd, wc0, wc1, wc2}[col] * (-ln 2)
     float bd, bc[3], sat;
-    alignas(16) float edf[kP3Warps][32 * kEdfStride];         // (EDF mode only; last member) edf[ray][col] = 2^(zf), zf = -log2(e) * dir_net(SH16(d))[col]
 };
 
-__device__ __forceinline__ void split2_p3(float x0, float x1, uint32_t& hi, uint32_t& lo) {   // packed converts (F2FP), not 4 scalar F2F
-    const __half2 h = __floats2half2_rn(x0, x1);
-    const float2 hf = __half22float2(h);
-    const __half2 l = __floats2half2_rn(x0 - hf.x, x1 - hf.y);
-    hi = *reinterpret_cast<const uint32_t*>(&h);
-    lo = *reinterpret_cast<const uint32_t*>(&l);
-}
-__device__ __forceinline__ void ldmatrix_x4_p3(uint32_t addr, uint32_t* r) {
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void mma_16816_p3(float* d, const uint32_t* a, uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
-// EDF = true: exp(-f) table in shared memory, one ex2 per hidden unit (3 CTAs / SM by shared memory);
-// EDF = false: no table -- both exponentials evaluated, 33 KB of shared memory per CTA so occupancy is set by registers alone.
-// ABL: timing-only ablations (SSDNERF_P3_ABLATE, wrong images): 1 = no transcendentals in the heads, 2 = no plane gather, 3 = no MMA, 4 = no probe arithmetic
-template <int MINB, bool EDF, int ABL>
-__global__ void __launch_bounds__(kP3Threads, MINB) k_render_p3(RenderParams p, int mode) {
+// persistent CTAs; each warp takes 32-ray tiles from counters[mode]
+// mode 0: main pass (cap = max_steps + 7, builds the lifetime histogram)
+// mode 1: fix-up pass (only rays whose main-pass count exceeds the emulated budget are re-rendered)
+__global__ void __launch_bounds__(kP3Threads, 3) k_render_p3(RenderParams p, int mode) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     SmemP3& s = *reinterpret_cast<SmemP3*>(smem_raw);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int g = lane >> 2, t4 = lane & 3;
+    const int t4 = lane & 3;
     {   // ---- stage weights once per (persistent) CTA
         const float* blob = p.blob;
         // W[n][k], k = plane*8 + c (c < 6) | k = 24: bias | else 0; stored directly as mma B fragments (hi and lo halves)
@@ -84,7 +59,7 @@ __global__ void __launch_bounds__(kP3Threads, MINB) k_render_p3(RenderParams p, 
                     else if (k == kOneK3) v[e] = __ldg(blob + DecP::OFF_B1 + n);
                     v[e] *= -kLog2e;                 // the MMA delivers z = -log2(e) * pre-activation
                 }
-                split2_p3(v[0], v[1], hi[w], lo[w]);
+                split2(v[0], v[1], hi[w], lo[w]);
             }
             s.wfrag[nt][0][ln] = make_uint4(hi[0], hi[1], hi[2], hi[3]);
             s.wfrag[nt][1][ln] = make_uint4(lo[0], lo[1], lo[2], lo[3]);
@@ -104,7 +79,7 @@ __global__ void __launch_bounds__(kP3Threads, MINB) k_render_p3(RenderParams p, 
                     if (k == 0) v[e] += __ldg(blob + DecP::OFF_BDIR + n) * (1.0f / 0.28209479177387814f);
                     v[e] *= -kLog2e;
                 }
-                split2_p3(v[0], v[1], hi[w], lo[w]);
+                split2(v[0], v[1], hi[w], lo[w]);
             }
             s.dfrag[nt][ln] = make_uint4(hi[0], hi[1], lo[0], lo[1]);
         }
@@ -130,7 +105,6 @@ __global__ void __launch_bounds__(kP3Threads, MINB) k_render_p3(RenderParams p, 
     const uint32_t a_lo_base = (uint32_t)__cvta_generic_to_shared(s.a_lo[warp]);
     // ldmatrix row address of this lane for (m-tile mt, k-chunk kc): row 16*mt + lane%16, column byte offset (16*kc + (lane/16)*8)*2
     const uint32_t ld_off = (uint32_t)((lane & 15) * kARow3 + (lane >> 4) * 16);
-    float* edfw = s.edf[warp];
 
     const uint32_t tiles_per_scene = div_up(p.rays_per_scene, 32u);
     const uint32_t total_tiles = tiles_per_scene * p.num_scenes;
@@ -161,7 +135,7 @@ __global__ void __launch_bounds__(kP3Threads, MINB) k_render_p3(RenderParams p, 
         MarchCfg c = p.cfg;
         if (p.dt_gamma) c.dt_gamma = __ldg(p.dt_gamma + scene);
 
-        // per-ray view-direction features: SH16(d) as split-fp16 A fragments (registers, whole tile) and edf[ray][col] = 2^(zf)
+        // per-ray view-direction features: SH16(d) as split-fp16 A fragments (registers, whole tile)
         uint32_t ash[2][4], asl[2][4];
         {
             float sh[16];
@@ -171,37 +145,20 @@ __global__ void __launch_bounds__(kP3Threads, MINB) k_render_p3(RenderParams p, 
 #pragma unroll
             for (int q = 0; q < 2; ++q) {
                 uint4 vh, vl;
-                split2_p3(sh[8 * q], sh[8 * q + 1], vh.x, vl.x);
-                split2_p3(sh[8 * q + 2], sh[8 * q + 3], vh.y, vl.y);
-                split2_p3(sh[8 * q + 4], sh[8 * q + 5], vh.z, vl.z);
-                split2_p3(sh[8 * q + 6], sh[8 * q + 7], vh.w, vl.w);
+                split2(sh[8 * q], sh[8 * q + 1], vh.x, vl.x);
+                split2(sh[8 * q + 2], sh[8 * q + 3], vh.y, vl.y);
+                split2(sh[8 * q + 4], sh[8 * q + 5], vh.z, vl.z);
+                split2(sh[8 * q + 6], sh[8 * q + 7], vh.w, vl.w);
                 rh[q] = vh; rl[q] = vl;
             }
             __syncwarp();
 #pragma unroll
             for (int mt = 0; mt < 2; ++mt) {
-                ldmatrix_x4_p3(a_hi_base + mt * 16 * kARow3 + ld_off, ash[mt]);
-                ldmatrix_x4_p3(a_lo_base + mt * 16 * kARow3 + ld_off, asl[mt]);
+                ldmatrix_x4(a_hi_base + mt * 16 * kARow3 + ld_off, ash[mt]);
+                ldmatrix_x4(a_lo_base + mt * 16 * kARow3 + ld_off, asl[mt]);
             }
             __syncwarp();
-            // columns 0..23 of the A rows are rewritten by every sample; restore the zero padding lanes 6, 7 of each plane group now
-            // (feature rows store 0 there anyway) -- nothing to do.  edf table:
-#pragma unroll 1
-            for (int nt = 0; EDF && nt < 8; ++nt) {
-                const uint4 bd4 = s.dfrag[nt][lane];
-#pragma unroll
-                for (int mt = 0; mt < 2; ++mt) {
-                    float zf[4] = {0.f, 0.f, 0.f, 0.f};
-                    mma_16816_p3(zf, asl[mt], bd4.x, bd4.y);
-                    mma_16816_p3(zf, ash[mt], bd4.z, bd4.w);
-                    mma_16816_p3(zf, ash[mt], bd4.x, bd4.y);
-                    const int col = nt * 8 + 2 * t4;
-                    *reinterpret_cast<float2*>(edfw + (g + 16 * mt) * kEdfStride + col) = make_float2(ex2_approx(zf[0]), ex2_approx(zf[1]));
-                    *reinterpret_cast<float2*>(edfw + (g + 16 * mt + 8) * kEdfStride + col) = make_float2(ex2_approx(zf[2]), ex2_approx(zf[3]));
-                }
-            }
         }
-        __syncwarp();
 
         const float* planes = reinterpret_cast<const float*>(p.planes) + (size_t)scene * 3 * p.plane_h * p.plane_w * DecP::CPAD;
         const size_t plane_stride = (size_t)p.plane_h * p.plane_w * DecP::CPAD;
@@ -218,35 +175,24 @@ __global__ void __launch_bounds__(kP3Threads, MINB) k_render_p3(RenderParams p, 
             float x = 0.0f, y = 0.0f, z = 0.0f, dt = 0.0f; uint32_t vi = 0;
             while (alive && !has) {
                 if (!(t < far) || ns >= cap) { alive = false; break; }
-                if (ABL == 4) { x = fmaf(t, r.dx, r.ox); y = fmaf(t, r.dy, r.oy); z = fmaf(t, r.dz, r.oz); dt = c.dt_min; vi = 0; has = true; }
-                else has = probe(c, r, grid, t, x, y, z, dt, vi);
+                has = probe(c, r, grid, t, x, y, z, dt, vi);
             }
-            const unsigned has_mask = __ballot_sync(0xffffffffu, has);
-            if (!has_mask) break;
-            if (p.prof && lane == 0) {       // debug instrumentation (NULL in production): lane utilisation of the decode iterations
-                atomicAdd(p.prof, 1ULL);
-                atomicAdd(p.prof + 1, (unsigned long long)__popc(has_mask));
-            }
+            if (!__ballot_sync(0xffffffffu, has)) break;
 
             // ---- phase 2: bilinear features of this lane's sample -> split fp16 row of the warp's A tile
             if (has) {
                 float f[DecP::KF];
-                if (ABL == 2) {
-#pragma unroll
-                    for (int q = 0; q < DecP::KF; ++q) f[q] = x * (float)q + y;
-                } else {
-                    gather_plane_p(planes, p.plane_h, p.plane_w, x, y, f);
-                    gather_plane_p(planes + plane_stride, p.plane_h, p.plane_w, x, z, f + 6);
-                    gather_plane_p(planes + 2 * plane_stride, p.plane_h, p.plane_w, y, z, f + 12);
-                }
+                gather_plane_p(planes, p.plane_h, p.plane_w, x, y, f);
+                gather_plane_p(planes + plane_stride, p.plane_h, p.plane_w, x, z, f + 6);
+                gather_plane_p(planes + 2 * plane_stride, p.plane_h, p.plane_w, y, z, f + 12);
                 uint4* rh = reinterpret_cast<uint4*>(s.a_hi[warp] + lane * kARow3);
                 uint4* rl = reinterpret_cast<uint4*>(s.a_lo[warp] + lane * kARow3);
 #pragma unroll
                 for (int pl = 0; pl < 3; ++pl) {
                     uint4 vh, vl;
-                    split2_p3(f[6 * pl], f[6 * pl + 1], vh.x, vl.x);
-                    split2_p3(f[6 * pl + 2], f[6 * pl + 3], vh.y, vl.y);
-                    split2_p3(f[6 * pl + 4], f[6 * pl + 5], vh.z, vl.z);
+                    split2(f[6 * pl], f[6 * pl + 1], vh.x, vl.x);
+                    split2(f[6 * pl + 2], f[6 * pl + 3], vh.y, vl.y);
+                    split2(f[6 * pl + 4], f[6 * pl + 5], vh.z, vl.z);
                     vh.w = 0; vl.w = 0;
                     rh[pl] = vh; rl[pl] = vl;
                 }
@@ -259,10 +205,10 @@ __global__ void __launch_bounds__(kP3Threads, MINB) k_render_p3(RenderParams p, 
             for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
                 for (int kc = 0; kc < 2; ++kc) {
-                    ldmatrix_x4_p3(a_hi_base + mt * 16 * kARow3 + kc * 32 + ld_off, ah[mt][kc]);
-                    ldmatrix_x4_p3(a_lo_base + mt * 16 * kARow3 + kc * 32 + ld_off, al[mt][kc]);
+                    ldmatrix_x4(a_hi_base + mt * 16 * kARow3 + kc * 32 + ld_off, ah[mt][kc]);
+                    ldmatrix_x4(a_lo_base + mt * 16 * kARow3 + kc * 32 + ld_off, al[mt][kc]);
                 }
-            // per-row partial head sums of this lane; rows g + 8*j, j = 0..3 (j = 2*mt + upper half)
+            // per-row partial head sums of this lane; rows lane / 4 + 8*j, j = 0..3 (j = 2*mt + upper half)
             float psd[4] = {0.f, 0.f, 0.f, 0.f}, pr[4] = {0.f, 0.f, 0.f, 0.f}, pg[4] = {0.f, 0.f, 0.f, 0.f}, pb[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll 1
             for (int nt = 0; nt < 8; ++nt) {
@@ -272,22 +218,16 @@ __global__ void __launch_bounds__(kP3Threads, MINB) k_render_p3(RenderParams p, 
 #pragma unroll
                 for (int mt = 0; mt < 2; ++mt) {
                     d[mt][0] = d[mt][1] = d[mt][2] = d[mt][3] = 0.0f;
-                    if (ABL == 3) {
-                        d[mt][0] = __uint_as_float(ah[mt][0][0] ^ bh.x); d[mt][1] = __uint_as_float(al[mt][1][1] ^ bl.y);
-                        d[mt][2] = __uint_as_float(ah[mt][1][2] ^ bh.z); d[mt][3] = __uint_as_float(al[mt][0][3] ^ bl.w);
-                        dc[mt][0] = d[mt][1] + __uint_as_float(bd4.x); dc[mt][1] = d[mt][0]; dc[mt][2] = d[mt][3]; dc[mt][3] = d[mt][2] + __uint_as_float(asl[mt][0]);
-                        continue;
-                    }
-                    mma_16816_p3(d[mt], al[mt][0], bh.x, bh.y);       // small terms first
-                    mma_16816_p3(d[mt], al[mt][1], bh.z, bh.w);
-                    mma_16816_p3(d[mt], ah[mt][0], bl.x, bl.y);
-                    mma_16816_p3(d[mt], ah[mt][1], bl.z, bl.w);
-                    mma_16816_p3(d[mt], ah[mt][0], bh.x, bh.y);
-                    mma_16816_p3(d[mt], ah[mt][1], bh.z, bh.w);
+                    mma_16816(d[mt], al[mt][0], make_uint2(bh.x, bh.y));       // small terms first
+                    mma_16816(d[mt], al[mt][1], make_uint2(bh.z, bh.w));
+                    mma_16816(d[mt], ah[mt][0], make_uint2(bl.x, bl.y));
+                    mma_16816(d[mt], ah[mt][1], make_uint2(bl.z, bl.w));
+                    mma_16816(d[mt], ah[mt][0], make_uint2(bh.x, bh.y));
+                    mma_16816(d[mt], ah[mt][1], make_uint2(bh.z, bh.w));
                     dc[mt][0] = d[mt][0]; dc[mt][1] = d[mt][1]; dc[mt][2] = d[mt][2]; dc[mt][3] = d[mt][3];
-                    mma_16816_p3(dc[mt], asl[mt], bd4.x, bd4.y);
-                    mma_16816_p3(dc[mt], ash[mt], bd4.z, bd4.w);
-                    mma_16816_p3(dc[mt], ash[mt], bd4.x, bd4.y);
+                    mma_16816(dc[mt], asl[mt], make_uint2(bd4.x, bd4.y));
+                    mma_16816(dc[mt], ash[mt], make_uint2(bd4.z, bd4.w));
+                    mma_16816(dc[mt], ash[mt], make_uint2(bd4.x, bd4.y));
                 }
                 const int col = nt * 8 + 2 * t4;
                 const float4 hw0 = s.heads[col], hw1 = s.heads[col + 1];
@@ -295,34 +235,19 @@ __global__ void __launch_bounds__(kP3Threads, MINB) k_render_p3(RenderParams p, 
                 for (int j = 0; j < 4; ++j) {
                     float z0 = d[j >> 1][(j & 1) * 2], z1 = d[j >> 1][(j & 1) * 2 + 1];          // -log2(e) * b
                     float y0 = dc[j >> 1][(j & 1) * 2], y1 = dc[j >> 1][(j & 1) * 2 + 1];        // -log2(e) * (b + f)
-                    float s0, s1, h0, h1;                                                         // z * sigmoid; the -ln 2 lives in the head weights
-                    if (ABL == 1) {            // ablation (timing only): no transcendental work
-                        s0 = fmaxf(z0, 0.f); s1 = fmaxf(z1, 0.f); h0 = fmaxf(y0, 0.f); h1 = fmaxf(y1, 0.f);
-                    } else if (EDF) {
-                        // exp(-b) once per unit; exp(-(b + f)) = exp(-b) exp(-f); every factor clamped to 2^30 so the 4-way product is finite
-                        const float2 ef = *reinterpret_cast<const float2*>(edfw + (g + 8 * j) * kEdfStride + col);
-                        const float e0 = ex2_approx(fminf(z0, 30.0f)), e1 = ex2_approx(fminf(z1, 30.0f));
-                        const float d1 = 1.0f + e0, d2 = 1.0f + e1;
-                        const float d3 = 1.0f + fminf(e0 * ef.x, 1073741824.0f), d4 = 1.0f + fminf(e1 * ef.y, 1073741824.0f);
-                        const float p12 = d1 * d2, p34 = d3 * d4;
-                        const float rr = rcp_approx(p12 * p34);
-                        const float r12 = rr * p34, r34 = rr * p12;            // 1 / (d1 d2), 1 / (d3 d4)
-                        s0 = z0 * (r12 * d2); s1 = z1 * (r12 * d1);
-                        h0 = y0 * (r34 * d4); h1 = y1 * (r34 * d3);
-                    } else {
-                        const float d1 = 1.0f + ex2_approx(fminf(z0, 60.0f)), d2 = 1.0f + ex2_approx(fminf(z1, 60.0f));
-                        const float d3 = 1.0f + ex2_approx(fminf(y0, 60.0f)), d4 = 1.0f + ex2_approx(fminf(y1, 60.0f));
-                        const float r12 = rcp_approx(d1 * d2), r34 = rcp_approx(d3 * d4);
-                        s0 = z0 * (r12 * d2); s1 = z1 * (r12 * d1);
-                        h0 = y0 * (r34 * d4); h1 = y1 * (r34 * d3);
-                    }
+                    // z * sigmoid (the -ln 2 lives in the head weights); exponents clamped to 60 so d1 * d2 stays finite
+                    const float d1 = 1.0f + ex2_approx(fminf(z0, 60.0f)), d2 = 1.0f + ex2_approx(fminf(z1, 60.0f));
+                    const float d3 = 1.0f + ex2_approx(fminf(y0, 60.0f)), d4 = 1.0f + ex2_approx(fminf(y1, 60.0f));
+                    const float r12 = rcp_approx(d1 * d2), r34 = rcp_approx(d3 * d4);
+                    const float s0 = z0 * (r12 * d2), s1 = z1 * (r12 * d1);
+                    const float h0 = y0 * (r34 * d4), h1 = y1 * (r34 * d3);
                     psd[j] = fmaf(s0, hw0.x, psd[j]);
                     psd[j] = fmaf(s1, hw1.x, psd[j]);
                     pr[j] = fmaf(h0, hw0.y, pr[j]); pg[j] = fmaf(h0, hw0.z, pg[j]); pb[j] = fmaf(h0, hw0.w, pb[j]);
                     pr[j] = fmaf(h1, hw1.y, pr[j]); pg[j] = fmaf(h1, hw1.z, pg[j]); pb[j] = fmaf(h1, hw1.w, pb[j]);
                 }
             }
-            // reduce over the 4 lanes of the quad (columns), then lane 4g+j keeps row g+8j and ships it to the owning lane
+            // reduce over the 4 lanes of the quad (columns), then lane 4g+j keeps row g+8j (g = 0..7) and ships it to the owning lane
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
 #pragma unroll
@@ -372,6 +297,7 @@ __global__ void __launch_bounds__(kP3Threads, MINB) k_render_p3(RenderParams p, 
             if (trace) for (uint32_t i = ns; i < p.trace_cap; ++i) trace[i] = -1;
             p.count_buf[gidx] = (int32_t)ns;
             if (mode == 0 && p.hist) {
+                // lifetime L: ray is still alive after a quantum ending at cumulative budget c iff L >= c
                 const uint32_t L = tbreak ? ns - 1 : ns;
                 atomicAdd(p.hist + (size_t)scene * p.hist_bins + min(L, p.hist_bins - 1), 1u);
             }
@@ -379,48 +305,25 @@ __global__ void __launch_bounds__(kP3Threads, MINB) k_render_p3(RenderParams p, 
     }
 }
 
-template <int MINB, bool EDF, int ABL>
-static int p3_launch(const RenderParams& p, int emulate_schedule, uint32_t* hist, int sms, cudaStream_t stream) {
-    const size_t smem = EDF ? sizeof(SmemP3) : offsetof(SmemP3, edf);
-    auto kern = k_render_p3<MINB, EDF, ABL>;
+int render_p3_launch(const RenderParams& p, int emulate_schedule, uint32_t* hist, int sms, cudaStream_t stream) {
+    const size_t smem = sizeof(SmemP3);
     static DeviceOnce attr_set;
     if (attr_set.first()) {
-        SSDNERF_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        SSDNERF_CUDA_OK(cudaFuncSetAttribute(k_render_p3, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
     int occ = 0;
-    SSDNERF_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kP3Threads, smem));
-    if (occ < 1) return set_error_msg(SSDNERF_ERR_CUDA, "render_fwd: variant P (mma v2) kernel does not fit on this device");
+    SSDNERF_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_render_p3, kP3Threads, smem));
+    if (occ < 1) return set_error_msg(SSDNERF_ERR_CUDA, "render_fwd: variant P kernel does not fit on this device");
     const uint32_t total_tiles = div_up(p.rays_per_scene, 32u) * p.num_scenes;
     const uint32_t grid = (uint32_t)min((uint64_t)sms * occ, (uint64_t)div_up(total_tiles, (uint32_t)kP3Warps));
-    kern<<<grid, kP3Threads, smem, stream>>>(p, 0);
+    k_render_p3<<<grid, kP3Threads, smem, stream>>>(p, 0);
     SSDNERF_LAUNCH_OK();
     if (emulate_schedule) {
         if (int e = launch_schedule(hist, p.hist_bins, p.num_scenes, p.rays_per_scene, p.max_steps, p.budget, stream)) return e;
-        kern<<<grid, kP3Threads, smem, stream>>>(p, 1);
+        k_render_p3<<<grid, kP3Threads, smem, stream>>>(p, 1);
         SSDNERF_LAUNCH_OK();
     }
     return 0;
-}
-
-// SSDNERF_P3_MODE = "noedf3" (default: no table, 3 CTAs / SM) | "noedf4" (<= 128 registers, 4 CTAs / SM) | "edf3" (exp table); A/B runs
-int render_p3_launch(const RenderParams& p, int emulate_schedule, uint32_t* hist, int sms, cudaStream_t stream) {
-    static int mode = -1;
-    if (mode < 0) {
-        const char* e = getenv("SSDNERF_P3_MODE");
-        mode = 1;      // noedf3; the three modes have not been compared on the H100
-        if (e) mode = !strcmp(e, "edf3") ? 0 : !strcmp(e, "noedf3") ? 1 : !strcmp(e, "noedf4") ? 2 : 1;
-    }
-    static int abl = -1;
-    if (abl < 0) { const char* e = getenv("SSDNERF_P3_ABLATE"); abl = e ? atoi(e) : 0; }
-    if (abl == 1) return p3_launch<3, false, 1>(p, emulate_schedule, hist, sms, stream);
-    if (abl == 2) return p3_launch<3, false, 2>(p, emulate_schedule, hist, sms, stream);
-    if (abl == 3) return p3_launch<3, false, 3>(p, emulate_schedule, hist, sms, stream);
-    if (abl == 4) return p3_launch<3, false, 4>(p, emulate_schedule, hist, sms, stream);
-    switch (mode) {
-        case 0: return p3_launch<3, true, 0>(p, emulate_schedule, hist, sms, stream);
-        case 2: return p3_launch<4, false, 0>(p, emulate_schedule, hist, sms, stream);
-        default: return p3_launch<3, false, 0>(p, emulate_schedule, hist, sms, stream);
-    }
 }
 
 }  // namespace ssdnerf

@@ -1,5 +1,5 @@
-// Fused inference renderer, variant S (3x32 channels, hidden 128, colour net 144 -> 128 -> 3), warp-synchronous version
-// (SSDNERF_DEC_S_MMA).  Same idea as render_p2.cu: every warp owns 32 rays, nothing is synchronised across warps.
+// Fused inference renderer, variant S (3x32 channels, hidden 128, colour net 144 -> 128 -> 3): the kernel behind SSDNERF_DEC_S.
+// Every warp owns 32 rays, nothing is synchronised across warps.
 //   * gather: four lanes cooperate on one sample (fp16 channels-last planes, 64 B per texel) and store their 8 interpolated
 //     channels straight into the warp's [32 x 96] fp16 A tile in shared memory;
 //   * GEMM1 (96 -> 128) on warp-level tensor-core MMAs (mma.sync.m16n8k16, fp16 x fp16 -> fp32); + b1, SiLU; the accumulator
@@ -16,39 +16,21 @@ namespace ssdnerf {
 constexpr int kS2Warps = 4, kS2Threads = kS2Warps * 32;
 constexpr int kS2ARow = 208;              // bytes per A1 row: 96 halves + 16 B pad (conflict-free ldmatrix)
 constexpr int kS2ShRow = 48;              // bytes per SH row: 16 halves + 16 B pad
-constexpr int kS2KF = 96, kS2Hid = 128, kS2K2 = 144;
-// blob offsets (render_common.cuh::DecS)
-constexpr int kS2OffW1 = 0, kS2OffB1 = kS2Hid * kS2KF, kS2OffWd = kS2OffB1 + kS2Hid, kS2OffBd = kS2OffWd + kS2Hid,
-              kS2OffWc0 = kS2OffBd + 4, kS2OffBc0 = kS2OffWc0 + kS2Hid * kS2K2, kS2OffWc2 = kS2OffBc0 + kS2Hid,
-              kS2OffBc2 = kS2OffWc2 + 3 * kS2Hid, kS2OffSat = kS2OffBc2 + 4;
 
 struct SmemS2 {
     alignas(16) uint2 w1f[16][6][32];        // GEMM1 B fragments [n-tile][k-chunk][lane] = {b0, b1}
     alignas(16) uint2 w2f[17][9][32];        // GEMM2 B fragments; n-tile 16 = density column (col 0) + zeros
     alignas(16) uint8_t a1[kS2Warps][32 * kS2ARow];
     alignas(16) uint8_t sh[kS2Warps][32 * kS2ShRow];
-    alignas(16) float b1[kS2Hid];
-    alignas(16) float b2[kS2Hid];
-    alignas(16) float4 wc2[kS2Hid];          // {wc0, wc1, wc2, 0}[col]
+    alignas(16) float b1[DecS::HID];
+    alignas(16) float b2[DecS::HID];
+    alignas(16) float4 wc2[DecS::HID];       // {wc0, wc1, wc2, 0}[col]
     float bd, bc2[3], sat;
 };
 
 __device__ __forceinline__ float s2_tanh(float x) { float y; asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float s2_silu(float x) { const float h = 0.5f * x; return fmaf(h, s2_tanh(h), h); }
 __device__ __forceinline__ uint32_t s2_pack(float a, float b) { const __half2 h = __floats2half2_rn(a, b); return *reinterpret_cast<const uint32_t*>(&h); }
-__device__ __forceinline__ void s2_ldmatrix_x4(uint32_t addr, uint32_t* r) {
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void s2_mma(float* d, const uint32_t* a, uint2 b) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b.x), "r"(b.y));
-}
-
-struct S2Grid {
-    const uint8_t* __restrict__ g;
-    __device__ __forceinline__ uint32_t operator()(uint32_t byte) const { return __ldg(g + byte); }
-};
-
 // 8 interpolated channels [8*sub, 8*sub+8) of plane texels around (u, v), as 8 packed halves
 __device__ __forceinline__ uint4 s2_gather(const __half* __restrict__ plane, uint32_t Hp, uint32_t Wp, float u, float v, int sub) {
     float ix = __fmul_rn(__fsub_rn(__fmul_rn(__fadd_rn(u, 1.0f), (float)Wp), 1.0f), 0.5f);
@@ -83,13 +65,13 @@ __global__ void __launch_bounds__(kS2Threads, 2) k_render_s2(RenderParams p, int
     extern __shared__ __align__(16) unsigned char smem_raw[];
     SmemS2& s = *reinterpret_cast<SmemS2*>(smem_raw);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int g = lane >> 2, t4 = lane & 3;
+    const int t4 = lane & 3;
     {   // ---- stage weights as mma B fragments (fp16), once per persistent CTA
         const float* blob = p.blob;
         for (int i = tid; i < 16 * 6 * 32; i += kS2Threads) {
             const int ln = i & 31, kc = (i >> 5) % 6, nt = i / (32 * 6);
             const int n = nt * 8 + (ln >> 2), k0 = kc * 16 + 2 * (ln & 3);
-            const float* w = blob + kS2OffW1 + n * kS2KF;          // W1[n][k], k = plane*32 + c
+            const float* w = blob + DecS::OFF_W1 + n * DecS::KF;          // W1[n][k], k = plane*32 + c
             s.w1f[nt][kc][ln] = make_uint2(s2_pack(__ldg(w + k0), __ldg(w + k0 + 1)), s2_pack(__ldg(w + k0 + 8), __ldg(w + k0 + 9)));
         }
         for (int i = tid; i < 17 * 9 * 32; i += kS2Threads) {
@@ -99,21 +81,21 @@ __global__ void __launch_bounds__(kS2Threads, 2) k_render_s2(RenderParams p, int
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
                 const int k = k0 + (e & 1) + (e >> 1) * 8;
-                if (n < kS2Hid) v[e] = __ldg(blob + kS2OffWc0 + n * kS2K2 + k);              // colour hidden layer: [base_act | SH16]
-                else if (n == kS2Hid && k < kS2Hid) v[e] = __ldg(blob + kS2OffWd + k);       // density column reads base_act only
+                if (n < DecS::HID) v[e] = __ldg(blob + DecS::OFF_WC0 + n * DecS::K2 + k);              // colour hidden layer: [base_act | SH16]
+                else if (n == DecS::HID && k < DecS::HID) v[e] = __ldg(blob + DecS::OFF_WD + k);       // density column reads base_act only
                 else v[e] = 0.0f;
             }
             s.w2f[nt][kc][ln] = make_uint2(s2_pack(v[0], v[1]), s2_pack(v[2], v[3]));
         }
-        for (int i = tid; i < kS2Hid; i += kS2Threads) {
-            s.b1[i] = __ldg(blob + kS2OffB1 + i);
-            s.b2[i] = __ldg(blob + kS2OffBc0 + i);
-            s.wc2[i] = make_float4(__ldg(blob + kS2OffWc2 + i), __ldg(blob + kS2OffWc2 + kS2Hid + i), __ldg(blob + kS2OffWc2 + 2 * kS2Hid + i), 0.0f);
+        for (int i = tid; i < DecS::HID; i += kS2Threads) {
+            s.b1[i] = __ldg(blob + DecS::OFF_B1 + i);
+            s.b2[i] = __ldg(blob + DecS::OFF_BC0 + i);
+            s.wc2[i] = make_float4(__ldg(blob + DecS::OFF_WC2 + i), __ldg(blob + DecS::OFF_WC2 + DecS::HID + i), __ldg(blob + DecS::OFF_WC2 + 2 * DecS::HID + i), 0.0f);
         }
         if (tid == 0) {
-            s.bd = __ldg(blob + kS2OffBd);
-            s.bc2[0] = __ldg(blob + kS2OffBc2); s.bc2[1] = __ldg(blob + kS2OffBc2 + 1); s.bc2[2] = __ldg(blob + kS2OffBc2 + 2);
-            s.sat = __ldg(blob + kS2OffSat);
+            s.bd = __ldg(blob + DecS::OFF_BD);
+            s.bc2[0] = __ldg(blob + DecS::OFF_BC2); s.bc2[1] = __ldg(blob + DecS::OFF_BC2 + 1); s.bc2[2] = __ldg(blob + DecS::OFF_BC2 + 2);
+            s.sat = __ldg(blob + DecS::OFF_SAT);
         }
         uint4* r0 = reinterpret_cast<uint4*>(s.a1[warp] + lane * kS2ARow);
 #pragma unroll
@@ -172,7 +154,7 @@ __global__ void __launch_bounds__(kS2Threads, 2) k_render_s2(RenderParams p, int
 
         const __half* planes = reinterpret_cast<const __half*>(p.planes) + (size_t)scene * 3 * p.plane_h * p.plane_w * 32;
         const size_t plane_stride = (size_t)p.plane_h * p.plane_w * 32;
-        S2Grid grid{p.bitfield + (size_t)scene * (p.cfg.H * p.cfg.H * p.cfg.H / 8) * p.cfg.C};
+        BitfieldLoader grid{p.bitfield + (size_t)scene * (p.cfg.H * p.cfg.H * p.cfg.H / 8) * p.cfg.C};
         int32_t* trace = p.voxel_trace ? p.voxel_trace + gidx * p.trace_cap : nullptr;
 
         float t = near;
@@ -216,7 +198,7 @@ __global__ void __launch_bounds__(kS2Threads, 2) k_render_s2(RenderParams p, int
 #pragma unroll
                 for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
-                    for (int kc = 0; kc < 6; ++kc) s2_ldmatrix_x4(a1_base + mt * 16 * kS2ARow + kc * 32 + ld_off_a, a1f[mt][kc]);
+                    for (int kc = 0; kc < 6; ++kc) ldmatrix_x4(a1_base + mt * 16 * kS2ARow + kc * 32 + ld_off_a, a1f[mt][kc]);
 #pragma unroll
                 for (int kc2 = 0; kc2 < 8; ++kc2) {
 #pragma unroll
@@ -227,7 +209,7 @@ __global__ void __launch_bounds__(kS2Threads, 2) k_render_s2(RenderParams p, int
                         for (int mt = 0; mt < 2; ++mt) {
                             d[mt][0] = d[mt][1] = d[mt][2] = d[mt][3] = 0.0f;
 #pragma unroll
-                            for (int kc = 0; kc < 6; ++kc) s2_mma(d[mt], a1f[mt][kc], s.w1f[nt][kc][lane]);
+                            for (int kc = 0; kc < 6; ++kc) mma_16816(d[mt], a1f[mt][kc], s.w1f[nt][kc][lane]);
                         }
                         const float2 bb = *reinterpret_cast<const float2*>(s.b1 + nt * 8 + 2 * t4);
 #pragma unroll
@@ -241,7 +223,7 @@ __global__ void __launch_bounds__(kS2Threads, 2) k_render_s2(RenderParams p, int
             // ---- phase 4: GEMM2 ([base_act | SH16] -> 128 hidden + density) with the 128 -> 3 layer on the accumulator fragments
             uint32_t shf[2][4];
 #pragma unroll
-            for (int mt = 0; mt < 2; ++mt) s2_ldmatrix_x4(sh_base + mt * 16 * kS2ShRow + ld_off_s, shf[mt]);
+            for (int mt = 0; mt < 2; ++mt) ldmatrix_x4(sh_base + mt * 16 * kS2ShRow + ld_off_s, shf[mt]);
             float pr[4] = {0.f, 0.f, 0.f, 0.f}, pg[4] = {0.f, 0.f, 0.f, 0.f}, pb[4] = {0.f, 0.f, 0.f, 0.f}, psd[4];
 #pragma unroll 1
             for (int nt = 0; nt < 17; ++nt) {
@@ -250,8 +232,8 @@ __global__ void __launch_bounds__(kS2Threads, 2) k_render_s2(RenderParams p, int
                 for (int mt = 0; mt < 2; ++mt) {
                     d[mt][0] = d[mt][1] = d[mt][2] = d[mt][3] = 0.0f;
 #pragma unroll
-                    for (int kc = 0; kc < 8; ++kc) s2_mma(d[mt], a2[mt][kc], s.w2f[nt][kc][lane]);
-                    s2_mma(d[mt], shf[mt], s.w2f[nt][8][lane]);
+                    for (int kc = 0; kc < 8; ++kc) mma_16816(d[mt], a2[mt][kc], s.w2f[nt][kc][lane]);
+                    mma_16816(d[mt], shf[mt], s.w2f[nt][8][lane]);
                 }
                 if (nt < 16) {
                     const int col = nt * 8 + 2 * t4;

@@ -429,9 +429,9 @@ extern "C" {
 static int train_launch(const ssdnerf_render_train_args* a, bool bwd, cudaStream_t stream) {
     const bool wg = bwd && a && a->grad_decoder_blob;
     if (!a) return set_error_msg(SSDNERF_ERR_ARG, "render_train: args is NULL");
-    if (a->num_scenes == 0 || a->rays_per_scene == 0) return 0;
-    if (a->variant != SSDNERF_DEC_P && a->variant != SSDNERF_DEC_P_SIMT && a->variant != SSDNERF_DEC_P_MMA && a->variant != SSDNERF_DEC_P_MMA2)
+    if (a->variant != SSDNERF_DEC_P)
         return set_error_msg(SSDNERF_ERR_ARG, "render_train: only decoder variant P has a fused differentiable renderer");
+    if (a->num_scenes == 0 || a->rays_per_scene == 0) return 0;
     if (!a->rays_o || !a->rays_d || !a->planes || !a->bitfield || !a->decoder_blob || !a->image || !a->weights_sum || !a->counter)
         return set_error_msg(SSDNERF_ERR_ARG, "render_train: rays, planes, bitfield, decoder_blob, image, weights_sum and counter are required");
     if (bwd && (!a->grad_image || !a->grad_planes)) return set_error_msg(SSDNERF_ERR_ARG, "render_train_bwd: grad_image and grad_planes are required");

@@ -6,7 +6,7 @@ Plugin surface of lib/models/decoders/base_volume_renderer.py:11-133 and triplan
 return_loss)` returning `dict(weights_sum, depth, image)` as per-scene lists in eval mode, `point_decode`,
 `point_density_decode`, attributes `bound / min_near / max_steps / aabb`.
 
-eval mode (`self.training == False`): ONE fused launch sequence (csrc/render_fused.cu, csrc/render_p3.cu, csrc/render_s2.cu).
+eval mode (`self.training == False`): ONE fused launch sequence (csrc/render.cu, csrc/render_p3.cu, csrc/render_s2.cu).
 train mode: decoder of the shipped-config shape -> fused differentiable renderer (csrc/render_train.cu): gradient w.r.t. the
 code (guidance / code optimisation with a frozen decoder, diffusion_nerf.py:273) and, when the decoder is trainable (stage-1
 auto-decoder training, multiscene_nerf.py:159-252), w.r.t. its weights.  `point_decode` / `point_density_decode` are one native launch (csrc/point_decode.cu).

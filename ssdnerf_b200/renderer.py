@@ -10,11 +10,6 @@ from . import _lib as N
 
 DEC_P = 0   # shipped configs: base 18->64, density 64->1, dir_net 16->64, color 64->3
 DEC_S = 1   # TriPlaneDecoder class defaults: base 96->128, density 128->1, color 144->128->3
-DEC_P_SIMT = 2   # DEC_P on the CUDA cores (plain fp32)
-DEC_P_MMA = 4    # DEC_P, warp-synchronous split-precision mma.sync base layer
-DEC_S_MMA = 5    # DEC_S, warp-synchronous mma.sync kernel
-DEC_P_MMA2 = 7   # DEC_P, warp-synchronous v2 (shared exponentials, tensor-core dir_net): what DEC_P selects
-_VARIANT_C = {DEC_P: 6, DEC_S: 32, DEC_P_SIMT: 6, DEC_P_MMA: 6, DEC_S_MMA: 32, DEC_P_MMA2: 6}
 
 
 def detect_variant(params):
@@ -37,7 +32,7 @@ def _plane_major(w, C):
 
 
 def pack_decoder_blob(params, variant=None, sigmoid_saturation=0.001, device='cuda'):
-    """Flatten decoder weights into the fp32 blob the kernels read (layout documented in csrc/render_fused.cu
+    """Flatten decoder weights into the fp32 blob the kernels read (layout documented in csrc/dec_p.cuh
     `DecP` and csrc/render_common.cuh `DecS`)."""
     if variant is None:
         variant = detect_variant(params)
@@ -47,13 +42,13 @@ def pack_decoder_blob(params, variant=None, sigmoid_saturation=0.001, device='cu
     def pad(t, n):
         return torch.cat([t, torch.zeros(n, device=src)])
     tail = torch.tensor([sigmoid_saturation, 0, 0, 0], dtype=torch.float32, device=src)
-    if variant in (DEC_P, DEC_P_SIMT, DEC_P_MMA, DEC_P_MMA2):
+    if variant == DEC_P:
         w1 = _plane_major(p['base_net.0.weight'], 6).t().contiguous()           # [18][64], row k = plane*6+c
         parts = [w1.reshape(-1), p['base_net.0.bias'],
                  p['density_net.0.weight'].reshape(-1), pad(p['density_net.0.bias'], 3),
                  p['dir_net.0.weight'].t().contiguous().reshape(-1), p['dir_net.0.bias'],      # [16][64]
                  p['color_net.0.weight'].reshape(-1), pad(p['color_net.0.bias'], 1), tail]
-    elif variant in (DEC_S, DEC_S_MMA):
+    elif variant == DEC_S:
         w1 = _plane_major(p['base_net.0.weight'], 32)                             # [128][96] (N x K, K contiguous)
         wc0 = p['color_net.0.weight']                                             # [128][144]: cols 0..127 base_act, 128..143 SH
         parts = [w1.reshape(-1), p['base_net.0.bias'],
@@ -106,7 +101,7 @@ def pack_planes(code, variant):
 
 def render_fwd(variant, planes, plane_hw, bitfield, blob, rays_o=None, rays_d=None, poses=None, intrinsics=None,
                img_hw=None, grid_size=64, bound=1.0, min_near=0.2, max_steps=256, T_thresh=1e-4, bg_color=1.0,
-               dt_gamma=None, emulate_schedule=True, trace_cap=0, want_blend=True, want_counts=True, debug_phase_cycles=None):
+               dt_gamma=None, emulate_schedule=True, trace_cap=0, want_blend=True, want_counts=True):
     """One fused render of B scenes.
 
     Either explicit rays (rays_o, rays_d: [B,N,3]) or cameras (poses [B,V,4,4], intrinsics [B,V,4], img_hw).
@@ -151,7 +146,6 @@ def render_fwd(variant, planes, plane_hw, bitfield, blob, rays_o=None, rays_d=No
     a.weights_sum, a.depth, a.image = N.ptr(out['weights_sum']), N.ptr(out['depth']), N.ptr(out['image'])
     a.rgb_blend, a.num_samples = N.ptr(out['rgb']), N.ptr(out['num_samples'])
     a.voxel_trace, a.trace_cap = N.ptr(out['trace']), trace_cap
-    a.debug_phase_cycles = N.ptr(debug_phase_cycles)
     a.workspace, a.workspace_bytes = N.ptr(workspace), ws_bytes
     import ctypes
     N.check(N.lib().ssdnerf_render_fwd(ctypes.byref(a), N.stream_ptr()))

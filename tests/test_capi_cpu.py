@@ -34,6 +34,50 @@ def test_argument_errors_without_gpu():
     assert b'NULL' in L.ssdnerf_last_error()
 
 
+def test_unknown_decoder_variant_is_rejected_before_any_launch():
+    """only SSDNERF_DEC_P (0) and SSDNERF_DEC_S (1) exist; render_fwd rejects any other id before it enqueues work on the stream"""
+    from ssdnerf_b200 import _lib as N
+    L = N.lib()
+    u32 = ctypes.c_uint32
+    n, max_steps = 64 * 64, 256
+    ws_bytes = L.ssdnerf_render_workspace_bytes(u32(1), u32(n), u32(max_steps))
+    fake = ctypes.c_void_p(1 << 20)                  # never dereferenced: validation fails first
+    for v in (2, 4, 5, 7, -1):
+        assert L.ssdnerf_decoder_blob_floats(ctypes.c_int(v)) == 0
+        assert L.ssdnerf_planes_bytes(ctypes.c_int(v), u32(1), u32(128), u32(128)) == 0
+        assert L.ssdnerf_pack_planes(ctypes.c_int(v), None, u32(1), u32(6), u32(128), u32(128), None, None) == -2
+        a = N.RenderArgs()
+        a.variant, a.num_scenes, a.rays_per_scene = v, 1, n
+        a.rays_o = a.rays_d = a.planes = a.bitfield = a.decoder_blob = a.weights_sum = a.image = fake
+        a.plane_h = a.plane_w = 128
+        a.grid_size, a.bound, a.min_near, a.T_thresh, a.max_steps = 64, 1.0, 0.2, 1e-4, max_steps
+        a.workspace, a.workspace_bytes = fake, ws_bytes
+        assert L.ssdnerf_render_fwd(ctypes.byref(a), None) == -2, v
+        assert b'variant' in L.ssdnerf_last_error()
+
+
+def test_ctypes_arg_structs_match_header(tmp_path):
+    """RenderArgs / RenderTrainArgs mirror ssdnerf_render_args / ssdnerf_render_train_args field by field: the host compiler's
+    sizeof and offsetof for the header equal ctypes' layout"""
+    import subprocess
+    from ssdnerf_b200 import _lib as N
+    mirrors = {'ssdnerf_render_args': N.RenderArgs, 'ssdnerf_render_train_args': N.RenderTrainArgs}
+    lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "ssdnerf_b200.h"', 'int main(void) {']
+    expect = []
+    for cname, mirror in mirrors.items():
+        lines.append(f'    printf("%zu\\n", sizeof({cname}));')
+        expect.append(ctypes.sizeof(mirror))
+        for name, _ in mirror._fields_:
+            lines.append(f'    printf("%zu\\n", offsetof({cname}, {name}));')
+            expect.append(getattr(mirror, name).offset)
+    lines += ['    return 0;', '}']
+    src, exe = tmp_path / 'layout.c', tmp_path / 'layout'
+    src.write_text('\n'.join(lines) + '\n')
+    subprocess.run(['cc', '-I', os.path.join(ROOT, 'include'), '-o', str(exe), str(src)], check=True)
+    got = [int(x) for x in subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.split()]
+    assert got == expect
+
+
 def test_python_frontend_refuses_cpu_tensors():
     import pytest
     import torch

@@ -11,7 +11,7 @@ from tests.common import config1, spiral_poses
 
 pytestmark = pytest.mark.gpu
 
-# fp32 CUDA-core MLP (variant P): only round-off / fast-intrinsic differences vs the fp32 oracle
+# split-precision tensor-core MLP with fp32 accumulation (variant P): only round-off / fast-intrinsic differences vs the fp32 oracle
 TOL_P = dict(rtol=2e-4, atol=2e-5)
 # fp16 tensor-core MLP + fp16 planes (variant S): BASELINE.json north_star "1e-3 relative fp16 tolerance" on rendered RGB, taken on the
 # image range [0, 1]; the bar is half the stated tolerance.
@@ -21,7 +21,8 @@ TOL_S = dict(rtol=0, atol=5e-4)
 def _bitfields():
     ones = np.full(64 ** 3 // 8, 255, np.uint8)
     sphere = rp.sphere_bitfield()
-    return {'ones': ones, 'sphere': sphere}
+    rand = np.random.default_rng(0).integers(0, 256, 64 ** 3 // 8, dtype=np.uint8)   # ~half the cells: many empty / occupied switches
+    return {'ones': ones, 'sphere': sphere, 'random': rand}
 
 
 def _run_gpu(variant, vid, params, code, bf, poses, intr, res, cuda, max_steps, explicit, trace_cap):
@@ -41,16 +42,18 @@ def _run_gpu(variant, vid, params, code, bf, poses, intr, res, cuda, max_steps, 
     return {k: (v.cpu().numpy() if v is not None else None) for k, v in out.items()}
 
 
-@pytest.mark.parametrize('variant', ['P', 'P_SIMT', 'P_MMA', 'P_MMA2', 'S'])
-@pytest.mark.parametrize('grid', ['ones', 'sphere'])
-def test_config1_explicit_rays(cuda, variant, grid):
-    """SURVEY §8d config 1: 64x64 render, max_steps=32 (fixed step dt_max), bit-exact integer trace."""
+@pytest.mark.parametrize('variant', ['P', 'S'])
+@pytest.mark.parametrize('grid', ['ones', 'sphere', 'random'])
+@pytest.mark.parametrize('max_steps', [32, 256])
+def test_config1_explicit_rays(cuda, variant, grid, max_steps):
+    """SURVEY §8d config 1: 64x64 render, max_steps=32 (fixed step dt_max), bit-exact integer trace; also at the shipped
+    max_steps=256, where the emulated sample budget and the ray's exit from the box end the march instead."""
     from ssdnerf_b200 import renderer as R
-    vid = {'P': R.DEC_P, 'P_SIMT': R.DEC_P_SIMT, 'P_MMA': R.DEC_P_MMA, 'P_MMA2': R.DEC_P_MMA2, 'S': R.DEC_S}[variant]
+    vid = {'P': R.DEC_P, 'S': R.DEC_S}[variant]
     code, poses, intr = config1(variant[0])
     params = rp.make_decoder_params(variant[0], 0)
     bf = _bitfields()[grid]
-    res, max_steps = 64, 32
+    res = 64
     ro, rd = rp.get_cam_rays(poses[0], intr[0], res, res)
     ref = rp.render_eval_scene(params, ro.reshape(-1, 3).numpy(), rd.reshape(-1, 3).numpy(), code[0], bf, max_steps=max_steps,
                                return_trace=True)
