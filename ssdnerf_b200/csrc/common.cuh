@@ -103,11 +103,13 @@ __device__ __forceinline__ int mip_from_dt(float dt, float H, float max_cascade)
 // Per-launch marching constants (raymarching.cu:736-745).
 struct MarchCfg {
     float bound, dt_gamma, dt_min, dt_max, rH, H3f, Hf, Cf;
+    float rbound0;             // 1 / min(1, bound) (IEEE division): the mip_rbound of cascade 0, all `probe` needs when C == 1
     uint32_t H, C;
 };
 __host__ __device__ inline MarchCfg make_march_cfg(float bound, float dt_gamma, uint32_t max_steps, uint32_t C, uint32_t H) {
     MarchCfg c;
     c.bound = bound; c.dt_gamma = dt_gamma; c.H = H; c.C = C;
+    c.rbound0 = 1.0f / fminf(1.0f, bound);
     c.Hf = (float)H; c.Cf = (float)C;
     c.rH = 1.0f / (float)H;
     c.H3f = (float)(H * H * H);
@@ -168,12 +170,12 @@ __device__ __forceinline__ bool probe(const MarchCfg& c, const Ray& r, GridLoade
     z = clampf(__fmaf_rn(t0, r.dz, r.oz), -c.bound, c.bound);
     dt = clampf(__fmul_rn(t0, c.dt_gamma), c.dt_min, c.dt_max);
     int level = 0;
-    float mip_bound = fminf(1.0f, c.bound);
+    float mip_bound = fminf(1.0f, c.bound), mip_rbound = c.rbound0;
     if (c.C > 1) {
         level = max(mip_from_pos(x, y, z, c.Cf), mip_from_dt(dt, c.Hf, c.Cf));
         mip_bound = fminf(scalbnf(1.0f, level), c.bound);
+        mip_rbound = __fdiv_rn(1.0f, mip_bound);
     }
-    const float mip_rbound = __fdiv_rn(1.0f, mip_bound);
     const int nx = voxel_coord(x, mip_rbound, c);
     const int ny = voxel_coord(y, mip_rbound, c);
     const int nz = voxel_coord(z, mip_rbound, c);

@@ -2,15 +2,18 @@
 //
 // Every warp owns a tile of 32 rays and nothing is synchronised across warps. A lane marches its own ray through the occupancy grid,
 // gathers the 18 bilinear triplane features of its next sample and composites; the MLP runs on the tensor cores for the whole warp.
-//   * base layer 18 -> 64 as split-precision mma.sync: features and weights are each split into fp16 hi + lo halves and the three
-//     significant products (lo*hi, hi*lo, hi*hi) accumulate in fp32, which keeps fp32-class accuracy; the bias rides on a constant-one
-//     column of the A tile;
-//   * dir_net 16 -> 64 on the tensor cores on top of the base accumulator: the SH16 fragments of the ray direction stay in registers for
-//     the whole tile (bias folded into the constant SH basis 0), so the colour branch's pre-activation b + f comes out of the MMA;
+//   * base layer 18 -> 64 as one K = 64 split-precision mma.sync chain: features and weights are each split into fp16 hi + lo halves
+//     and the three significant products (hi*hi, lo*hi, hi*lo) sit side by side in one A row and one B column, so each (n-tile,
+//     m-tile) takes 4 MMAs; they accumulate in fp32, which keeps fp32-class accuracy.  The bias rides on two constant-one columns
+//     (hi and lo half of the bias);
+//   * dir_net 16 -> 64 depends on the ray only: when a warp takes a tile it evaluates -log2(e) * (Wdir SH16(d) + bdir) once per ray
+//     with split-precision MMAs and keeps it in shared memory in accumulator-fragment order, so the colour branch's pre-activation
+//     is the base accumulator plus 8 FADDs per n-tile;
 //   * -log2(e) is folded into the staged weights (the MMA delivers z = -log2(e) * pre-activation, the argument of ex2) and -ln 2 into the
 //     head weights, which takes the scaling multiplies out of the inner loop;
-//   * the density and colour heads are evaluated on the accumulator fragments: SiLU in pairs, two ex2 and one rcp per pair
-//     (one reciprocal of the product of the two denominators), then quad shuffles reduce over the columns.
+//   * the density and colour heads are evaluated on the accumulator fragments: SiLU in fours (the density and colour pre-activations
+//     of two columns of one row), four ex2 and one rcp of the product of the four denominators, then the quad reduce-scatters the
+//     head partials so that each lane holds one row.
 #include "common.cuh"
 #include "render_common.cuh"
 #include "dec_p.cuh"
@@ -20,17 +23,40 @@ namespace ssdnerf {
 
 constexpr float kLog2e = 1.4426950408889634f, kLn2 = 0.6931471805599453f;
 constexpr int kP3Warps = 4, kP3Threads = kP3Warps * 32;
-constexpr int kARow3 = 80;                // bytes per A-tile row: 32 halves + 16 B pad (conflict-free ldmatrix / 16-byte stores)
-constexpr int kOneK3 = 24;                // K index of the constant-one (bias) column
+// A row of the base layer, 64 halves: [hi f0..17, 1, 0 | lo f0..17 | hi f0..17, 1, 0 x 7] (segments at halves 0, 20 and 38; even
+// offsets, so every feature pair is one packed half2 word).  The matching B column is [Whi; bhi; 0 | Whi | Wlo; blo; 0 x 7].
+constexpr int kKSeg1 = 20, kKSeg2 = 38;
+constexpr int kARow3 = 144;               // bytes per A-tile row: 64 halves + 16 B pad (conflict-free ldmatrix / 16-byte stores)
+constexpr uint32_t kOneLo = 0x3C00u;      // half2 word (1.0, 0.0): the constant-one column and the zero after it
 
 struct SmemP3 {
-    alignas(16) uint8_t a_hi[kP3Warps][32 * kARow3];
-    alignas(16) uint8_t a_lo[kP3Warps][32 * kARow3];
-    alignas(16) uint4 wfrag[8][2][32];                         // base layer: [n-tile][hi|lo][lane] = {b0,b1 of k-chunk 0, b0,b1 of k-chunk 1}
+    alignas(16) uint8_t a[kP3Warps][32 * kARow3];
+    alignas(16) uint4 wfrag[8][2][32];                         // base layer: [n-tile][k-chunks 0,1 | 2,3][lane] = {b0,b1, b0,b1}
     alignas(16) uint4 dfrag[8][32];                            // dir_net: [n-tile][lane] = {b0,b1 hi, b0,b1 lo}, K = 16 SH values
+    alignas(16) float4 dirs[kP3Warps][8][2][32];               // per tile: -log2(e) * dir_net(SH16(d)) as [n-tile][m-tile][lane] fragments
     float4 heads[DecP::HID];                                   // {wd, wc0, wc1, wc2}[col] * (-ln 2)
     float bd, bc[3], sat;
 };
+
+// fp16 entry (k, n) of the base layer's B operand (see kKSeg1): hi or lo half of the scaled weight / bias
+__device__ __forceinline__ __half base_b(const float* __restrict__ blob, int k, int n) {
+    const int r = k < kKSeg1 ? k : (k < kKSeg2 ? k - kKSeg1 : k - kKSeg2);
+    float v = 0.0f;
+    if (r < DecP::KF) v = __ldg(blob + DecP::OFF_W1 + r * DecP::HID + n);
+    else if (r == DecP::KF && (k < kKSeg1 || k >= kKSeg2)) v = __ldg(blob + DecP::OFF_B1 + n);
+    v *= -kLog2e;                            // the MMA delivers z = -log2(e) * pre-activation
+    const __half hi = __float2half_rn(v);
+    return k < kKSeg2 ? hi : __float2half_rn(v - __half2float(hi));
+}
+
+// Sum of a[j] over the 4 lanes of a quad, scattered: lane t4 of the quad returns the total of a[t4]
+__device__ __forceinline__ float quad_reduce_scatter(const float (&a)[4], int t4) {
+    const bool up2 = t4 & 2, up1 = t4 & 1;
+    float b[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) b[i] = (up2 ? a[i + 2] : a[i]) + __shfl_xor_sync(0xffffffffu, up2 ? a[i] : a[i + 2], 2);
+    return (up1 ? b[1] : b[0]) + __shfl_xor_sync(0xffffffffu, up1 ? b[0] : b[1], 1);
+}
 
 // persistent CTAs; each warp takes 32-ray tiles from counters[mode]
 // mode 0: main pass (cap = max_steps + 7, builds the lifetime histogram)
@@ -42,27 +68,19 @@ __global__ void __launch_bounds__(kP3Threads, 3) k_render_p3(RenderParams p, int
     const int t4 = lane & 3;
     {   // ---- stage weights once per (persistent) CTA
         const float* blob = p.blob;
-        // W[n][k], k = plane*8 + c (c < 6) | k = 24: bias | else 0; stored directly as mma B fragments (hi and lo halves)
+        // base layer as mma B fragments: k = kc*16 + (b0|b1)*8 + 2*tt, +1 of column n
         for (int i = tid; i < 8 * 32; i += kP3Threads) {
             const int nt = i >> 5, ln = i & 31, gg = ln >> 2, tt = ln & 3;
             const int n = nt * 8 + gg;
-            uint32_t hi[4], lo[4];
+            uint32_t b[8];
 #pragma unroll
-            for (int w = 0; w < 4; ++w) {           // w = kc*2 + (b0|b1): k = kc*16 + (w&1)*8 + 2*tt, +1
-                float v[2];
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    const int k = (w >> 1) * 16 + (w & 1) * 8 + 2 * tt + e;
-                    const int pl = k >> 3, c = k & 7;
-                    v[e] = 0.0f;
-                    if (pl < 3 && c < DecP::C) v[e] = __ldg(blob + DecP::OFF_W1 + (pl * DecP::C + c) * DecP::HID + n);
-                    else if (k == kOneK3) v[e] = __ldg(blob + DecP::OFF_B1 + n);
-                    v[e] *= -kLog2e;                 // the MMA delivers z = -log2(e) * pre-activation
-                }
-                split2(v[0], v[1], hi[w], lo[w]);
+            for (int w = 0; w < 8; ++w) {           // w = kc*2 + (b0|b1)
+                const int k = (w >> 1) * 16 + (w & 1) * 8 + 2 * tt;
+                const __half2 h = __halves2half2(base_b(blob, k, n), base_b(blob, k + 1, n));
+                b[w] = *reinterpret_cast<const uint32_t*>(&h);
             }
-            s.wfrag[nt][0][ln] = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-            s.wfrag[nt][1][ln] = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+            s.wfrag[nt][0][ln] = make_uint4(b[0], b[1], b[2], b[3]);
+            s.wfrag[nt][1][ln] = make_uint4(b[4], b[5], b[6], b[7]);
         }
         // dir_net as B fragments, K = 16 SH basis values; SH basis 0 is the constant 0.28209479..., so the bias rides on its weight
         for (int i = tid; i < 8 * 32; i += kP3Threads) {
@@ -92,19 +110,18 @@ __global__ void __launch_bounds__(kP3Threads, 3) k_render_p3(RenderParams p, int
             s.bc[0] = __ldg(blob + DecP::OFF_BC); s.bc[1] = __ldg(blob + DecP::OFF_BC + 1); s.bc[2] = __ldg(blob + DecP::OFF_BC + 2);
             s.sat = __ldg(blob + DecP::OFF_SAT);
         }
-        // this lane's A rows: zero, then the constant-one column (hi = 1.0)
-        uint4* rh = reinterpret_cast<uint4*>(s.a_hi[warp] + lane * kARow3);
-        uint4* rl = reinterpret_cast<uint4*>(s.a_lo[warp] + lane * kARow3);
+        // this lane's A row: zero, then halves 56..63 = (1, 0 x 7), which no later store touches
+        uint4* row = reinterpret_cast<uint4*>(s.a[warp] + lane * kARow3);
 #pragma unroll
-        for (int i = 0; i < kARow3 / 16; ++i) { rh[i] = make_uint4(0, 0, 0, 0); rl[i] = make_uint4(0, 0, 0, 0); }
-        reinterpret_cast<__half*>(s.a_hi[warp] + lane * kARow3)[kOneK3] = __float2half(1.0f);
+        for (int i = 0; i < 7; ++i) row[i] = make_uint4(0, 0, 0, 0);
+        row[7] = make_uint4(kOneLo, 0, 0, 0);
     }
     __syncthreads();
 
-    const uint32_t a_hi_base = (uint32_t)__cvta_generic_to_shared(s.a_hi[warp]);
-    const uint32_t a_lo_base = (uint32_t)__cvta_generic_to_shared(s.a_lo[warp]);
+    const uint32_t a_base = (uint32_t)__cvta_generic_to_shared(s.a[warp]);
     // ldmatrix row address of this lane for (m-tile mt, k-chunk kc): row 16*mt + lane%16, column byte offset (16*kc + (lane/16)*8)*2
     const uint32_t ld_off = (uint32_t)((lane & 15) * kARow3 + (lane >> 4) * 16);
+    uint4* const my_row = reinterpret_cast<uint4*>(s.a[warp] + lane * kARow3);
 
     const uint32_t tiles_per_scene = div_up(p.rays_per_scene, 32u);
     const uint32_t total_tiles = tiles_per_scene * p.num_scenes;
@@ -135,13 +152,11 @@ __global__ void __launch_bounds__(kP3Threads, 3) k_render_p3(RenderParams p, int
         MarchCfg c = p.cfg;
         if (p.dt_gamma) c.dt_gamma = __ldg(p.dt_gamma + scene);
 
-        // per-ray view-direction features: SH16(d) as split-fp16 A fragments (registers, whole tile)
-        uint32_t ash[2][4], asl[2][4];
+        // per-ray view-direction term, once per tile: SH16(d) as split fp16 (hi at halves 0..15, lo at 16..31 of this lane's A row),
+        // dir_net on the tensor cores, the accumulator fragments parked in s.dirs for the column loop
         {
             float sh[16];
             sh16(r.dx, r.dy, r.dz, sh);
-            uint4* rh = reinterpret_cast<uint4*>(s.a_hi[warp] + lane * kARow3);
-            uint4* rl = reinterpret_cast<uint4*>(s.a_lo[warp] + lane * kARow3);
 #pragma unroll
             for (int q = 0; q < 2; ++q) {
                 uint4 vh, vl;
@@ -149,15 +164,28 @@ __global__ void __launch_bounds__(kP3Threads, 3) k_render_p3(RenderParams p, int
                 split2(sh[8 * q + 2], sh[8 * q + 3], vh.y, vl.y);
                 split2(sh[8 * q + 4], sh[8 * q + 5], vh.z, vl.z);
                 split2(sh[8 * q + 6], sh[8 * q + 7], vh.w, vl.w);
-                rh[q] = vh; rl[q] = vl;
+                my_row[q] = vh; my_row[2 + q] = vl;
             }
             __syncwarp();
+            uint32_t ash[2][4], asl[2][4];
 #pragma unroll
             for (int mt = 0; mt < 2; ++mt) {
-                ldmatrix_x4(a_hi_base + mt * 16 * kARow3 + ld_off, ash[mt]);
-                ldmatrix_x4(a_lo_base + mt * 16 * kARow3 + ld_off, asl[mt]);
+                ldmatrix_x4(a_base + mt * 16 * kARow3 + ld_off, ash[mt]);
+                ldmatrix_x4(a_base + mt * 16 * kARow3 + 32 + ld_off, asl[mt]);
             }
             __syncwarp();
+#pragma unroll 1
+            for (int nt = 0; nt < 8; ++nt) {
+                const uint4 bd4 = s.dfrag[nt][lane];
+#pragma unroll
+                for (int mt = 0; mt < 2; ++mt) {
+                    float dd[4] = {0.f, 0.f, 0.f, 0.f};
+                    mma_16816(dd, asl[mt], make_uint2(bd4.x, bd4.y));       // small terms first
+                    mma_16816(dd, ash[mt], make_uint2(bd4.z, bd4.w));
+                    mma_16816(dd, ash[mt], make_uint2(bd4.x, bd4.y));
+                    s.dirs[warp][nt][mt][lane] = make_float4(dd[0], dd[1], dd[2], dd[3]);
+                }
+            }
         }
 
         const float* planes = reinterpret_cast<const float*>(p.planes) + (size_t)scene * 3 * p.plane_h * p.plane_w * DecP::CPAD;
@@ -179,89 +207,70 @@ __global__ void __launch_bounds__(kP3Threads, 3) k_render_p3(RenderParams p, int
             }
             if (!__ballot_sync(0xffffffffu, has)) break;
 
-            // ---- phase 2: bilinear features of this lane's sample -> split fp16 row of the warp's A tile
+            // ---- phase 2: bilinear features of this lane's sample -> split fp16 A row (halves 0..55; 56..63 are constant)
             if (has) {
                 float f[DecP::KF];
                 gather_plane_p(planes, p.plane_h, p.plane_w, x, y, f);
                 gather_plane_p(planes + plane_stride, p.plane_h, p.plane_w, x, z, f + 6);
                 gather_plane_p(planes + 2 * plane_stride, p.plane_h, p.plane_w, y, z, f + 12);
-                uint4* rh = reinterpret_cast<uint4*>(s.a_hi[warp] + lane * kARow3);
-                uint4* rl = reinterpret_cast<uint4*>(s.a_lo[warp] + lane * kARow3);
+                uint32_t hi[9], lo[9];
 #pragma unroll
-                for (int pl = 0; pl < 3; ++pl) {
-                    uint4 vh, vl;
-                    split2(f[6 * pl], f[6 * pl + 1], vh.x, vl.x);
-                    split2(f[6 * pl + 2], f[6 * pl + 3], vh.y, vl.y);
-                    split2(f[6 * pl + 4], f[6 * pl + 5], vh.z, vl.z);
-                    vh.w = 0; vl.w = 0;
-                    rh[pl] = vh; rl[pl] = vl;
-                }
+                for (int i = 0; i < 9; ++i) split2(f[2 * i], f[2 * i + 1], hi[i], lo[i]);
+                my_row[0] = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+                my_row[1] = make_uint4(hi[4], hi[5], hi[6], hi[7]);
+                my_row[2] = make_uint4(hi[8], kOneLo, lo[0], lo[1]);
+                my_row[3] = make_uint4(lo[2], lo[3], lo[4], lo[5]);
+                my_row[4] = make_uint4(lo[6], lo[7], lo[8], hi[0]);
+                my_row[5] = make_uint4(hi[1], hi[2], hi[3], hi[4]);
+                my_row[6] = make_uint4(hi[5], hi[6], hi[7], hi[8]);
             }
             __syncwarp();
 
             // ---- phase 3: base layer on the tensor cores + heads on the accumulator fragments
-            uint32_t ah[2][2][4], al[2][2][4];          // [m-tile][k-chunk][a0..a3]
+            uint32_t a[2][4][4];                    // [m-tile][k-chunk][a0..a3]
 #pragma unroll
             for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
-                for (int kc = 0; kc < 2; ++kc) {
-                    ldmatrix_x4(a_hi_base + mt * 16 * kARow3 + kc * 32 + ld_off, ah[mt][kc]);
-                    ldmatrix_x4(a_lo_base + mt * 16 * kARow3 + kc * 32 + ld_off, al[mt][kc]);
-                }
+                for (int kc = 0; kc < 4; ++kc) ldmatrix_x4(a_base + mt * 16 * kARow3 + kc * 32 + ld_off, a[mt][kc]);
             // per-row partial head sums of this lane; rows lane / 4 + 8*j, j = 0..3 (j = 2*mt + upper half)
             float psd[4] = {0.f, 0.f, 0.f, 0.f}, pr[4] = {0.f, 0.f, 0.f, 0.f}, pg[4] = {0.f, 0.f, 0.f, 0.f}, pb[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll 1
+#pragma unroll
             for (int nt = 0; nt < 8; ++nt) {
-                const uint4 bh = s.wfrag[nt][0][lane], bl = s.wfrag[nt][1][lane];
-                const uint4 bd4 = s.dfrag[nt][lane];
+                const uint4 b01 = s.wfrag[nt][0][lane], b23 = s.wfrag[nt][1][lane];
                 float d[2][4], dc[2][4];            // z of the density branch, z of the colour branch (= base + dir_net)
 #pragma unroll
                 for (int mt = 0; mt < 2; ++mt) {
                     d[mt][0] = d[mt][1] = d[mt][2] = d[mt][3] = 0.0f;
-                    mma_16816(d[mt], al[mt][0], make_uint2(bh.x, bh.y));       // small terms first
-                    mma_16816(d[mt], al[mt][1], make_uint2(bh.z, bh.w));
-                    mma_16816(d[mt], ah[mt][0], make_uint2(bl.x, bl.y));
-                    mma_16816(d[mt], ah[mt][1], make_uint2(bl.z, bl.w));
-                    mma_16816(d[mt], ah[mt][0], make_uint2(bh.x, bh.y));
-                    mma_16816(d[mt], ah[mt][1], make_uint2(bh.z, bh.w));
-                    dc[mt][0] = d[mt][0]; dc[mt][1] = d[mt][1]; dc[mt][2] = d[mt][2]; dc[mt][3] = d[mt][3];
-                    mma_16816(dc[mt], asl[mt], make_uint2(bd4.x, bd4.y));
-                    mma_16816(dc[mt], ash[mt], make_uint2(bd4.z, bd4.w));
-                    mma_16816(dc[mt], ash[mt], make_uint2(bd4.x, bd4.y));
+                    mma_16816(d[mt], a[mt][2], make_uint2(b23.x, b23.y));      // small terms first: chunks 2, 3 hold only lo*hi, hi*lo, blo
+                    mma_16816(d[mt], a[mt][3], make_uint2(b23.z, b23.w));
+                    mma_16816(d[mt], a[mt][1], make_uint2(b01.z, b01.w));      // chunk 1: hi*hi of f16, f17 and the bias, lo*hi of f0..11
+                    mma_16816(d[mt], a[mt][0], make_uint2(b01.x, b01.y));      // chunk 0: hi*hi of f0..15
+                    const float4 dir = s.dirs[warp][nt][mt][lane];
+                    dc[mt][0] = d[mt][0] + dir.x; dc[mt][1] = d[mt][1] + dir.y; dc[mt][2] = d[mt][2] + dir.z; dc[mt][3] = d[mt][3] + dir.w;
                 }
                 const int col = nt * 8 + 2 * t4;
                 const float4 hw0 = s.heads[col], hw1 = s.heads[col + 1];
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
-                    float z0 = d[j >> 1][(j & 1) * 2], z1 = d[j >> 1][(j & 1) * 2 + 1];          // -log2(e) * b
-                    float y0 = dc[j >> 1][(j & 1) * 2], y1 = dc[j >> 1][(j & 1) * 2 + 1];        // -log2(e) * (b + f)
-                    // z * sigmoid (the -ln 2 lives in the head weights); exponents clamped to 60 so d1 * d2 stays finite
-                    const float d1 = 1.0f + ex2_approx(fminf(z0, 60.0f)), d2 = 1.0f + ex2_approx(fminf(z1, 60.0f));
-                    const float d3 = 1.0f + ex2_approx(fminf(y0, 60.0f)), d4 = 1.0f + ex2_approx(fminf(y1, 60.0f));
-                    const float r12 = rcp_approx(d1 * d2), r34 = rcp_approx(d3 * d4);
-                    const float s0 = z0 * (r12 * d2), s1 = z1 * (r12 * d1);
-                    const float h0 = y0 * (r34 * d4), h1 = y1 * (r34 * d3);
-                    psd[j] = fmaf(s0, hw0.x, psd[j]);
-                    psd[j] = fmaf(s1, hw1.x, psd[j]);
+                    const float z0 = d[j >> 1][(j & 1) * 2], z1 = d[j >> 1][(j & 1) * 2 + 1];          // -log2(e) * b
+                    const float y0 = dc[j >> 1][(j & 1) * 2], y1 = dc[j >> 1][(j & 1) * 2 + 1];        // -log2(e) * (b + f)
+                    // z * sigmoid (the -ln 2 lives in the head weights): one rcp of the product of the four denominators 1 + 2^z; the
+                    // exponents are clamped at 30 so that product stays below 2^121 (the clamp moves SiLU by at most |x| * 2^-30)
+                    const float e0 = ex2_approx(fminf(z0, 30.0f)), e1 = ex2_approx(fminf(z1, 30.0f));
+                    const float e2 = ex2_approx(fminf(y0, 30.0f)), e3 = ex2_approx(fminf(y1, 30.0f));
+                    const float dz1 = 1.0f + e1, dy1 = 1.0f + e3;
+                    const float pz = fmaf(e0, dz1, dz1), py = fmaf(e2, dy1, dy1);                   // (1 + e0)(1 + e1), (1 + e2)(1 + e3)
+                    const float rcp4 = rcp_approx(pz * py);
+                    const float rz = rcp4 * py, ry = rcp4 * pz;
+                    const float h0 = (y0 * dy1) * ry, h1 = fmaf(y1, e2, y1) * ry;
+                    psd[j] = fmaf(rz, fmaf(fmaf(z1, e0, z1), hw1.x, (z0 * dz1) * hw0.x), psd[j]);     // s0 w0 + s1 w1 = rz (z0 d1 w0 + z1 d0 w1)
                     pr[j] = fmaf(h0, hw0.y, pr[j]); pg[j] = fmaf(h0, hw0.z, pg[j]); pb[j] = fmaf(h0, hw0.w, pb[j]);
                     pr[j] = fmaf(h1, hw1.y, pr[j]); pg[j] = fmaf(h1, hw1.z, pg[j]); pb[j] = fmaf(h1, hw1.w, pb[j]);
                 }
             }
-            // reduce over the 4 lanes of the quad (columns), then lane 4g+j keeps row g+8j (g = 0..7) and ships it to the owning lane
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-#pragma unroll
-                for (int o = 1; o <= 2; o <<= 1) {
-                    psd[j] += __shfl_xor_sync(0xffffffffu, psd[j], o);
-                    pr[j] += __shfl_xor_sync(0xffffffffu, pr[j], o);
-                    pg[j] += __shfl_xor_sync(0xffffffffu, pg[j], o);
-                    pb[j] += __shfl_xor_sync(0xffffffffu, pb[j], o);
-                }
-            }
-            const float osd = t4 == 0 ? psd[0] : (t4 == 1 ? psd[1] : (t4 == 2 ? psd[2] : psd[3]));
-            const float orr = t4 == 0 ? pr[0] : (t4 == 1 ? pr[1] : (t4 == 2 ? pr[2] : pr[3]));
-            const float ogg = t4 == 0 ? pg[0] : (t4 == 1 ? pg[1] : (t4 == 2 ? pg[2] : pg[3]));
-            const float obb = t4 == 0 ? pb[0] : (t4 == 1 ? pb[1] : (t4 == 2 ? pb[2] : pb[3]));
+            // reduce over the 4 lanes of the quad (columns): lane 4g+j ends with row g+8j (g = 0..7) and ships it to the owning lane
+            const float osd = quad_reduce_scatter(psd, t4), orr = quad_reduce_scatter(pr, t4);
+            const float ogg = quad_reduce_scatter(pg, t4), obb = quad_reduce_scatter(pb, t4);
             const int src = 4 * (lane & 7) + (lane >> 3);          // row `lane` = g + 8j lives in lane 4g + j
             const float sd = __shfl_sync(0xffffffffu, osd, src) + s.bd;
             const float o_r = __shfl_sync(0xffffffffu, orr, src) + s.bc[0];
