@@ -97,11 +97,29 @@ def point_preacts(params, xyzs, dirs, code_single, dtype=None):
     return base_x, base_x + F.linear(sh, params['dir_net.0.weight'], params['dir_net.0.bias']), logit
 
 
-def point_decode(params, xyzs, dirs, code_single, density_only=False, sigmoid_saturation=0.001, dtype=None):
+class TruncExp(torch.autograd.Function):
+    """lib/ops/activation.py:8-22 (_trunc_exp): y = exp(x); dy/dx := clamp(y, 1e-6, 1e6).  Unlike the reference it keeps the input's
+    precision, so the float64 oracle stays float64."""
+
+    @staticmethod
+    def forward(ctx, x):
+        y = torch.exp(x)
+        ctx.save_for_backward(y)
+        return y
+
+    @staticmethod
+    def backward(ctx, g):
+        y, = ctx.saved_tensors
+        return g * y.clamp(min=1e-6, max=1e6)
+
+
+def point_decode(params, xyzs, dirs, code_single, density_only=False, sigmoid_saturation=0.001, dtype=None, trunc_exp=True):
     """triplane_decoder.py:119-179 for ONE scene. xyzs (M,3), dirs (M,3), code (3,C,h,w) -> sigmas (M,), rgbs (M,3).
 
     dtype: run the MLP (grid_sample, linears, SiLU, exp, sigmoid) in this precision, e.g. torch.float64 as the high-precision
-    reference of the float32 kernels; None keeps the inputs' precision.  The SH encoding of `dirs` is float32 either way."""
+    reference of the float32 kernels; None keeps the inputs' precision.  The SH encoding of `dirs` is float32 either way.
+    trunc_exp: the density activation is the reference's TruncExp, whose gradient is floored at 1e-6 (a density logit below
+    ln 1e-6 = -13.8 still passes gradient); False differentiates plain exp."""
     params, xyzs, code_single = _cast(params, xyzs, code_single, dtype)
     M = xyzs.shape[0]
     pc = F.grid_sample(code_single, xyz_transform(xyzs), mode='bilinear', padding_mode='border',
@@ -109,7 +127,8 @@ def point_decode(params, xyzs, dirs, code_single, density_only=False, sigmoid_sa
     pc = pc.permute(2, 1, 0).reshape(M, -1)                        # feature index = c*3 + plane
     base_x = F.linear(pc, params['base_net.0.weight'], params['base_net.0.bias'])
     base_act = F.silu(base_x)
-    sig = torch.exp(F.linear(base_act, params['density_net.0.weight'], params['density_net.0.bias'])).squeeze(-1)
+    logit = F.linear(base_act, params['density_net.0.weight'], params['density_net.0.bias'])
+    sig = (TruncExp.apply(logit) if trunc_exp else torch.exp(logit)).squeeze(-1)
     if density_only:
         return sig, None
     sh = torch.from_numpy(orc.sh_encode(dirs.numpy(), 4)).to(base_x.dtype)

@@ -26,9 +26,13 @@ def _as_dtype(params, dtype):
 
 
 def render_train_scene(params, code_single, rays_o, rays_d, bitfield, noises=None, grid_size=64, bound=1.0, min_near=0.2,
-                       max_steps=256, dt_gamma=0.0, T_thresh=1e-4, dtype=torch.float64):
+                       max_steps=256, dt_gamma=0.0, T_thresh=1e-4, dtype=torch.float64, trunc_exp=True, return_samples=False):
     """One scene. code_single (3,C,h,w) torch (may require grad); rays (N,3) float32 numpy; bitfield uint8 numpy.
-    Returns weights_sum (N,), depth (N,), image (N,3) as torch tensors connected to `code_single`."""
+    Returns weights_sum (N,), depth (N,), image (N,3) as torch tensors connected to `code_single`.
+    trunc_exp: density activation as in `render_port.point_decode` (the reference's TruncExp by default).
+    return_samples: also return a dict of the marched samples -- `xyzs`, `dirs` (M,3) float32 numpy, `grad_mask` (M,) bool numpy of
+    the samples K8 writes a gradient for (composited and not the one at which T drops below T_thresh) and `counts` (N,) int64
+    numpy of the samples each ray composites (K7's count, the crossing sample included)."""
     rays_o = np.ascontiguousarray(rays_o, np.float32)
     rays_d = np.ascontiguousarray(rays_d, np.float32)
     n = rays_o.shape[0]
@@ -42,9 +46,13 @@ def render_train_scene(params, code_single, rays_o, rays_d, bitfield, noises=Non
     m = int(counts.sum())
     if m == 0:
         z = code_single.sum() * 0
-        return z + torch.zeros(n, dtype=dtype), z + torch.zeros(n, dtype=dtype), z + torch.zeros(n, 3, dtype=dtype)
+        res = z + torch.zeros(n, dtype=dtype), z + torch.zeros(n, dtype=dtype), z + torch.zeros(n, 3, dtype=dtype)
+        if return_samples:
+            res = res + (dict(xyzs=xyzs[:0], dirs=dirs[:0], grad_mask=np.zeros(0, bool), counts=np.zeros(n, np.int64)),)
+        return res
     p = _as_dtype(params, dtype)
-    sig, rgb = rp.point_decode(p, torch.from_numpy(xyzs[:m]).to(dtype), torch.from_numpy(dirs[:m]), code_single.to(dtype))
+    sig, rgb = rp.point_decode(p, torch.from_numpy(xyzs[:m]).to(dtype), torch.from_numpy(dirs[:m]), code_single.to(dtype),
+                               trunc_exp=trunc_exp)
     smax = int(counts.max())
     s_idx = torch.arange(smax)[None, :]
     valid = s_idx < torch.from_numpy(counts)[:, None]                                   # (N,S)
@@ -63,7 +71,12 @@ def render_train_scene(params, code_single, rays_o, rays_d, bitfield, noises=Non
     alpha = (1 - torch.exp(-sg * dt)) * included
     T_before = torch.cat([torch.ones(n, 1, dtype=dtype), torch.cumprod(1 - alpha, dim=1)[:, :-1]], dim=1)
     w = alpha * T_before
-    return w.sum(1), (w * tt).sum(1), (w[..., None] * cl).sum(1)
+    res = w.sum(1), (w * tt).sum(1), (w[..., None] * cl).sum(1)
+    if return_samples:
+        grad_mask = np.zeros(m, bool)
+        grad_mask[idx[included & ~crossing].numpy()] = True
+        res = res + (dict(xyzs=xyzs[:m], dirs=dirs[:m], grad_mask=grad_mask, counts=included.sum(1).numpy().astype(np.int64)),)
+    return res
 
 
 def render_loss(params, code, rays_o, rays_d, targets, bitfields, noises=None, dt_gamma=None, bg_color=1.0, pixel_weight=1.0,

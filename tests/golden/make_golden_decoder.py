@@ -8,6 +8,11 @@ oracle's restatements `render_port.point_decode / render_eval_scene` and `train_
 test of the fused renderers is measured against).
 
     python tests/golden/make_golden_decoder.py          (needs /root/reference)
+
+A second entry point runs the same train branch in the regimes where its edge rules act -- TruncExp's gradient floor, the plane borders,
+non-square planes, a binding sample budget -- into tests/golden/reference_train_edges_v1.npz:
+
+    python tests/golden/make_golden_decoder.py --train-edges
 """
 import ctypes
 import os
@@ -151,8 +156,76 @@ def run_reference():
     return out
 
 
+# ---------------------------------------------------------------------------------------------------------------------------------------
+# Train branch in the regimes where the fused differentiable renderer's edge rules act (-> reference_train_edges_v1.npz):
+#   floor       density bias -22: every density logit far below ln 1e-6, so K8's gradient reaches the code only through TruncExp's floor
+#   ones        all-ones occupancy grid: samples fill the whole box and reach the plane borders (grid_sample padding_mode='border')
+#   plane96x160 non-square planes
+#   budget32    all-ones grid at max_steps 32: the per-ray sample budget of march_rays_train binds
+# `rays` per scene: the stored code gradient grows with the texels the rays touch, so the all-ones cases (about 170 samples a ray at
+# max_steps 256) use few rays and the fixture stays small.
+TRAIN_EDGE_CASES = dict(floor=dict(bias=-22.0, grids=('sphere0.7', 'sphere0.5'), hw=(128, 128), max_steps=256, rays=24),
+                        ones=dict(bias=1.0, grids=('ones', 'ones'), hw=(128, 128), max_steps=256, rays=10),
+                        plane96x160=dict(bias=1.0, grids=('sphere0.7', 'sphere0.5'), hw=(96, 160), max_steps=256, rays=24),
+                        budget32=dict(bias=1.0, grids=('ones', 'ones'), hw=(128, 128), max_steps=32, rays=12))
+TRAIN_EDGE_RES, TRAIN_EDGE_DT_GAMMA = 24, (0.0, 0.004)
+
+
+def train_edge_inputs(name):
+    """Inputs of one train-edge case (no reference needed): code [2,3,6,H,W], decoder params, rays [2,24*24,3], bitfields [2,G^3/8]."""
+    c = TRAIN_EDGE_CASES[name]
+    seed = 40 + sorted(TRAIN_EDGE_CASES).index(name)
+    g = torch.Generator().manual_seed(seed)
+    code = (torch.randn(2, 3, 6, *c['hw'], generator=g) * 0.7).clamp(-2, 2)
+    params = rp.make_decoder_params('P', seed)
+    params['density_net.0.bias'] = params['density_net.0.bias'] + c['bias']
+    res = TRAIN_EDGE_RES
+    f = 131.25 * res / 128
+    poses = torch.from_numpy(spiral_poses(2)).float()
+    intr = torch.tensor([f, f, res / 2, res / 2]).expand(2, 4).contiguous()
+    ro, rd = rp.get_cam_rays(poses, intr, res, res)
+    bits = np.stack([np.full(64 ** 3 // 8, 255, np.uint8) if gr == 'ones' else rp.sphere_bitfield(radius=float(gr[6:])) for gr in c['grids']])
+    return dict(seed=seed, code=code, params=params, rays_o=ro.reshape(2, -1, 3).contiguous(), rays_d=rd.reshape(2, -1, 3).contiguous(),
+                bits=bits, max_steps=c['max_steps'])
+
+
+def run_reference_train_edges():
+    tri = load_reference_decoder()
+    torch.Tensor.cuda = lambda self, *a, **k: self
+    out = {}
+    for name in sorted(TRAIN_EDGE_CASES):
+        inp = train_edge_inputs(name)
+        g = torch.Generator().manual_seed(1000 + inp['seed'])
+        dec = tri.TriPlaneDecoder(**dict(CFG['P'], max_steps=inp['max_steps']))
+        missing = dec.load_state_dict({k: torch.as_tensor(v) for k, v in inp['params'].items()}, strict=False)
+        assert set(missing.missing_keys) <= {'aabb'} and not missing.unexpected_keys, missing
+        dec.train()
+        n_all = inp['rays_o'].shape[1]
+        n_rays = TRAIN_EDGE_CASES[name]['rays']
+        sel = torch.stack([torch.randperm(n_all, generator=g)[:n_rays] for _ in range(2)])
+        ro_t = torch.stack([inp['rays_o'][b][sel[b]] for b in range(2)])
+        rd_t = torch.stack([inp['rays_d'][b][sel[b]] for b in range(2)])
+        code_t = inp['code'].clone().requires_grad_(True)
+        r = dec(ro_t, rd_t, code_t, torch.from_numpy(inp['bits']), 64, dt_gamma=torch.tensor(TRAIN_EDGE_DT_GAMMA), perturb=False, return_loss=True)
+        gi, gw = torch.randn(2, n_rays, 3, generator=g), torch.randn(2, n_rays, generator=g)
+        ((r['image'] * gi).sum() + (r['weights_sum'] * gw).sum()).backward()
+        out[f'{name}_sel'], out[f'{name}_gi'], out[f'{name}_gw'] = sel.numpy().astype(np.int16), gi.numpy(), gw.numpy()
+        for k in ('weights_sum', 'depth', 'image'):
+            out[f'{name}_{k}'] = r[k].detach().numpy()
+        gc = code_t.grad.numpy().reshape(-1)                  # sparse: only texels next to a sample receive gradient
+        nz = np.nonzero(gc)[0]
+        out[f'{name}_grad_code_idx_diff'], out[f'{name}_grad_code_val'] = np.diff(nz, prepend=0).astype(np.int32), gc[nz]
+        for k, p in dec.named_parameters():
+            out[f'{name}_grad_{k}'] = p.grad.numpy()
+    return out
+
+
 if __name__ == '__main__':
-    res = run_reference()
-    path = os.path.join(HERE, 'reference_decoder_v1.npz')
+    if '--train-edges' in sys.argv:
+        res = run_reference_train_edges()
+        path = os.path.join(HERE, 'reference_train_edges_v1.npz')
+    else:
+        res = run_reference()
+        path = os.path.join(HERE, 'reference_decoder_v1.npz')
     np.savez_compressed(path, **res)
     print({k: v.shape for k, v in res.items() if v.ndim}, os.path.getsize(path), 'bytes')

@@ -1,10 +1,12 @@
 """CHECKER (tests only): the train-branch renderer composed op by op -- this library's per-op kernels, which are bit-exact with the
 reference's own (tests/test_ref_gpu.py): near/far K1, march_rays_train K6, composite_rays_train K7/K8 -- around a plain PyTorch
-decode (grid_sample + Linear, autograd) of the shipped-config decoder.  It is the A/B partner of the fused differentiable renderer
-(csrc/render_train.cu); the product has no such composition (a trainable decoder raises)."""
+decode (grid_sample + Linear, autograd) of the shipped-config decoder.  Its density activation is the library's trunc_exp, pinned to the
+reference's TruncExp, so the comparison also holds where the density gradient is floored (logits below ln 1e-6).  It is the A/B partner
+of the fused differentiable renderer (csrc/render_train.cu); the product has no such composition (a trainable decoder raises)."""
 import torch
 import torch.nn.functional as F
 
+from ssdnerf_b200.activation import trunc_exp
 from ssdnerf_b200.raymarching import batch_composite_rays_train, batch_near_far_from_aabb, march_rays_train
 from ssdnerf_b200.shencoder import sh_encode
 
@@ -15,7 +17,7 @@ def torch_point_decode(params, xyz, dirs, code_single, sat=0.001):
     feat = F.grid_sample(code_single, grid, mode='bilinear', padding_mode='border', align_corners=False).squeeze(-2)
     feat = feat.permute(2, 1, 0).reshape(xyz.shape[0], -1)
     base = F.linear(feat, params['base_net.0.weight'], params['base_net.0.bias'])
-    sigma = torch.exp(F.linear(F.silu(base), params['density_net.0.weight'], params['density_net.0.bias'])).squeeze(-1)
+    sigma = trunc_exp(F.linear(F.silu(base), params['density_net.0.weight'], params['density_net.0.bias'])).squeeze(-1)
     h = F.silu(base + F.linear(sh_encode(dirs, 4, False), params['dir_net.0.weight'], params['dir_net.0.bias']))
     rgb = torch.sigmoid(F.linear(h, params['color_net.0.weight'], params['color_net.0.bias']))
     return sigma, rgb * (1 + 2 * sat) - sat

@@ -1,4 +1,5 @@
 """CPU suite for the oracle: golden fixtures (tests/golden/oracle_v1.npz, made by make_golden.py) + domain properties."""
+import math
 import os
 
 import numpy as np
@@ -188,6 +189,10 @@ def test_train_render_gradient_finite_differences():
     code = code[None].double()
     loss, grad, out = tp.render_loss_grad(params, code, ro[None], rd[None], target, [bf], **kw)
     assert float(loss) > 0 and float(grad.abs().max()) > 0
+    # a gradient clamped by TruncExp's floor is not a derivative: every sample that passes gradient must sit above the floor
+    *_, smp = tp.render_train_scene(params, code[0], ro, rd, bf, noises, return_samples=True)
+    _, _, logit = rp.point_preacts(params, torch.from_numpy(smp['xyzs']), torch.from_numpy(smp['dirs']), code[0], dtype=torch.float64)
+    assert smp['grad_mask'].sum() > 100 and float(logit[torch.from_numpy(smp['grad_mask'])].min()) > math.log(1e-6) + 1
     flat = grad.reshape(-1)
     idx = torch.argsort(flat.abs(), descending=True)[:6]
     eps = 1e-5

@@ -506,3 +506,84 @@ def test_density_oracle_matches_reference_execution():
         _close(grid2[:, ::37], D[f'ue_grid_sub_{i}'], 2e-6 * float(D[f'ue_grid_sub_{i}'].max()) + 1e-7)
         diff = np.unpackbits(bits2) != np.unpackbits(D[f'ue_bits_{i}'])
         assert diff.mean() <= 2e-5, (i, diff.mean())
+
+
+def _train_edges_module():
+    import importlib.util
+    spec = importlib.util.spec_from_file_location('make_golden_decoder', os.path.join(GOLDEN, 'make_golden_decoder.py'))
+    mod = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(mod)
+    return mod
+
+
+@pytest.mark.parametrize('name', ['floor', 'ones', 'plane96x160', 'budget32'])
+def test_train_oracle_matches_reference_at_the_edges(name):
+    """`train_port.render_train_scene` vs the reference's own `TriPlaneDecoder` train branch (tests/golden/make_golden_decoder.py
+    --train-edges) where its edge rules act: TruncExp's gradient floor (density bias -22), the plane borders (all-ones grid), 96 x 160
+    planes and a binding sample budget (max_steps 32).  Forward to 5e-6, code and all eight decoder-parameter gradients to relative L2
+    2e-5.  At the floor the reference's float32 alpha is exactly 0 and the density path is the floor alone; the float64 oracle's alpha is
+    not, and it differs from float32 by about 1e-4 there, so that case is pinned with the oracle run in float32, the reference's own
+    precision."""
+    from oracle import train_port as tp
+    M = _train_edges_module()
+    D = np.load(os.path.join(GOLDEN, 'reference_train_edges_v1.npz'))
+    inp = M.train_edge_inputs(name)
+    dtype = torch.float32 if name == 'floor' else torch.float64
+    sel = torch.from_numpy(D[f'{name}_sel'].astype(np.int64))
+    gi, gw = torch.from_numpy(D[f'{name}_gi']).to(dtype), torch.from_numpy(D[f'{name}_gw']).to(dtype)
+    gcode = np.zeros(inp['code'].numel(), np.float32)
+    gcode[np.cumsum(D[f'{name}_grad_code_idx_diff'])] = D[f'{name}_grad_code_val']
+    gcode = gcode.reshape(inp['code'].shape)
+
+    def run(trunc_exp):
+        pref = {k: torch.as_tensor(v).to(dtype).requires_grad_(True) for k, v in inp['params'].items()}
+        cref = inp['code'].to(dtype).requires_grad_(True)
+        tot, outs = 0, []
+        for b in range(2):
+            ws, dep, img, smp = tp.render_train_scene(pref, cref[b], inp['rays_o'][b][sel[b]].numpy(), inp['rays_d'][b][sel[b]].numpy(), inp['bits'][b],
+                                                      None, dt_gamma=M.TRAIN_EDGE_DT_GAMMA[b], max_steps=inp['max_steps'], dtype=dtype,
+                                                      trunc_exp=trunc_exp, return_samples=True)
+            outs.append((ws, dep, img, smp))
+            tot = tot + (img * gi[b]).sum() + (ws * gw[b]).sum()
+        names = [k for k in pref if f'{name}_grad_{k}' in D.files]
+        return outs, dict(zip(['code'] + names, torch.autograd.grad(tot, [cref] + [pref[k] for k in names])))
+
+    def rel(a, b):
+        nb = float(np.linalg.norm(b))
+        return float((a.double() - torch.from_numpy(b).double()).norm()) / max(nb, 1e-30)
+
+    outs, grads = run(True)
+    assert len(grads) == 9
+    for b, (ws, dep, img, smp) in enumerate(outs):
+        for k, v in (('weights_sum', ws), ('depth', dep), ('image', img)):
+            _close(v.detach(), D[f'{name}_{k}'][b], 5e-6)
+    assert rel(grads['code'], gcode) < 2e-5, rel(grads['code'], gcode)
+    for k in list(grads)[1:]:
+        assert rel(grads[k], D[f'{name}_grad_{k}']) < 2e-5, (k, rel(grads[k], D[f'{name}_grad_{k}']))
+    # each case is in the regime it is named for
+    counts = np.concatenate([smp['counts'] for *_, smp in outs])
+    if name == 'budget32':
+        assert (counts == 32).mean() >= 0.25, (counts == 32).mean()
+    else:
+        assert counts.max() < inp['max_steps']
+    if name == 'floor':
+        assert float(np.abs(D['floor_weights_sum']).max()) == 0.0          # float32 alpha underflows to 0: the floor drives every gradient
+        _, grads_exp = run(False)                                        # plain exp's gradient misses the reference by far
+        k = 'density_net.0.bias'
+        assert rel(grads_exp[k], D[f'{name}_grad_{k}']) > 0.5, rel(grads_exp[k], D[f'{name}_grad_{k}'])
+    if name in ('ones', 'budget32'):
+        assert float(D[f'{name}_weights_sum'].max()) > 0.5
+    if name == 'ones':                                                   # samples within half a texel of a plane edge
+        xyzs = np.concatenate([smp['xyzs'] for *_, smp in outs])
+        assert (np.abs(xyzs) > 1 - 1 / 128).any(axis=1).mean() >= 0.01
+
+
+def test_oracle_trunc_exp_matches_reference_executed(ref):
+    """the oracle's TruncExp (render_port.point_decode's density activation) is bit-equal to the reference's _trunc_exp, forward and
+    backward, on the fixture's inputs, which straddle both clamp bounds of the gradient"""
+    from oracle.render_port import TruncExp
+    x = torch.from_numpy(ref['trunc_exp_x']).clone().requires_grad_(True)
+    y = TruncExp.apply(x)
+    y.backward(torch.ones_like(y))
+    assert np.array_equal(y.detach().numpy(), ref['trunc_exp_y']) and np.array_equal(x.grad.numpy(), ref['trunc_exp_grad'])
+    assert (ref['trunc_exp_x'] < np.log(1e-6)).any() and (ref['trunc_exp_x'] > np.log(1e6)).any()
