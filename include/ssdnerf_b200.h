@@ -258,7 +258,10 @@ typedef struct ssdnerf_gemm_args {
     float* qstats; uint32_t stats_hw;
     void* debug_cycles;      /* optional uint64[8] device counters of the generic tile kernel, clock cycles summed over CTAs: [0] producer wait
                               * for a free stage, [1] producer total, [2] consumer wait for a full stage, [4] consumer total; NULL in production */
-    uint32_t algo;           /* 0 = auto, 1 = generic tile kernel, 2 = row-pair 3x3 convolution (128-pixel rows, 128 output channels) */
+    uint32_t algo;           /* 0 = auto, 1 = generic tile kernel, 2 = row-pair 3x3 convolution (128-pixel rows, 128 output channels),
+                              * 3 = narrow-channel family: k1 / k2 multiples of 8 (a source's last K chunk is a short slab, only its
+                              * k-steps that hold data are issued), N tiles of 16 / 40 / 48 / 80 / 160 / 256 fitted to n (bn 0 = auto),
+                              * no clusters */
     /* generalised K-slabs: taps in [1, 9] with tap_offsets[2t], [2t+1] = shift of slab t in (d1, d2) (NULL: the 3x3 / 1x1 defaults) --
      * e.g. the four 2x2-tap phase convolutions a nearest-x2 upsample + 3x3 convolution decomposes into;
      * a_stride 2 = stride-2 convolution: (d1, d2) are output extents, a1 / a2 describe the (2 d1 x 2 d2) input read at every 2nd pixel */

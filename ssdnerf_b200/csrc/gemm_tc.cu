@@ -12,6 +12,10 @@
 //   epilogue (bias / residual / GroupNorm quad statistics / store) straight from the accumulator fragments while the producer already
 //   fills the stages of the next tile.
 // * clusters of CL = 2 / 4 / 8 CTAs along M: each CTA fetches 1/CL of the B (weight) tile and TMA-multicasts it to the whole cluster.
+// * narrow-channel family (KT = true, algo 3; the tiled-triplane UNet's 80 / 160 / 320 channels and 40 / 80-wide attention heads):
+//   K extents per source are multiples of 8 instead of 64.  A source's last 64-wide K chunk is a short slab: TMA zero-fills the box
+//   beyond the tensor map's K extent and the consumers issue only the ceil(valid / 16) k-steps that hold data.  The N tile is one of
+//   16 / 40 / 48 / 80 / 160 / 256 columns (any multiple of 8 is a legal wgmma N), picked to cover N exactly where possible.
 //
 // Replaces on the reference path: cuDNN Conv2d 3x3/1x1, Conv1d qkv/proj and the attention einsums of
 // lib/models/architecture/ddpm/{denoising,modules}.py (+ mmgen 0.7.2 blocks), see ssdnerf_b200/unet.py.
@@ -52,6 +56,7 @@ struct GemmParams {
     uint32_t stats_hw;          // > 0: image index of a row = (row index along d1) / stats_hw; 0: image index = index along d3
     unsigned long long* prof;   // optional debug counters (clock cycles summed over CTAs): [0] producer wait-empty, [1] producer total,
                                 // [2] consumer wait-full (warpgroup 1), [4] consumer total (warpgroup 1)
+    uint32_t k1, k2;            // narrow family only: K elements per tap of A1 / A2 (the B operand holds them back to back)
 };
 
 // CL = cluster size: 1 = single CTA; 2 / 4 / 8 = multicast cluster (every CTA loads 1/CL of the B tile and multicasts it to all)
@@ -68,7 +73,7 @@ struct GemmCfg {
 // The large layers are bound by operand delivery (L2 -> shared memory) rather than by the tensor cores: a 128 x BN tile re-fetches
 // (128 + BN) x 128 B per 64-wide k-block.  Wide N tiles (BN = 256, two consumer warpgroups of 64 x 256) amortise the A tile best;
 // multicast clusters additionally cut the B (weight) traffic by CL.
-template <int BN, int CL>
+template <int BN, int CL, bool KT>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 k_gemm_tc(const __grid_constant__ CUtensorMap mapA1, const __grid_constant__ CUtensorMap mapA2,
           const __grid_constant__ CUtensorMap mapB, const GemmParams p) {
@@ -123,10 +128,13 @@ k_gemm_tc(const __grid_constant__ CUtensorMap mapA1, const __grid_constant__ CUt
                         else mbar_wait(&empty[stage], phase ^ 1);
                         const bool first = j < p.kc1;
                         const int ak = (int)((first ? j : j - p.kc1) * kBK), a1 = (int)(t1 * p.b1 * p.a_stride) + ox, a2 = (int)(t2 * p.b2 * p.a_stride) + oy, a3 = (int)(t3 * p.b3);
-                        mbar_expect_tx(&full[stage], (uint32_t)Cfg::kStageBytes);
+                        mbar_expect_tx(&full[stage], (uint32_t)Cfg::kStageBytes);     // zero-filled box elements count too
                         tma_load_4d(sA + stage * kABytes, first ? &mapA1 : &mapA2, &full[stage], ak, a1, a2, a3);
+                        // B holds the two sources' K ranges back to back: with 64-aligned extents that is chunk j * 64, a short first
+                        // source shifts the second one's chunks to k1 + (j - kc1) * 64
+                        const int bk = KT ? (first ? ak : (int)p.k1 + ak) : (int)(j * kBK);
                         if (CL == 1) {
-                            tma_load_4d(sB + stage * Cfg::kBBytes, &mapB, &full[stage], (int)(j * kBK), (int)(n_tile * BN),
+                            tma_load_4d(sB + stage * Cfg::kBBytes, &mapB, &full[stage], bk, (int)(n_tile * BN),
                                         p.b_batched ? (int)t2 : (int)tap, p.b_batched ? (int)t3 : 0);
                         } else {   // this CTA's 1/CL slice of the B tile, broadcast to the whole cluster
                             tma_load_4d_mc(sB + stage * Cfg::kBBytes + crank * Cfg::kBoxRowsB * 128, &mapB, &full[stage], (int)(j * kBK),
@@ -159,6 +167,7 @@ k_gemm_tc(const __grid_constant__ CUtensorMap mapA1, const __grid_constant__ CUt
 #pragma unroll
             for (int i = 0; i < BN / 2; ++i) acc[i] = 0.0f;
             uint32_t prev = 0;
+            uint32_t jc = 0;                              // KT: chunk index within the current tap
             for (uint32_t it = 0; it < iters; ++it) {
                 if (p.prof && cw == 0) { const long long c = clock64(); mbar_wait(&full[stage], phase); wf += clock64() - c; }
                 else mbar_wait(&full[stage], phase);
@@ -166,10 +175,22 @@ k_gemm_tc(const __grid_constant__ CUtensorMap mapA1, const __grid_constant__ CUt
                 const uint64_t b_desc = make_desc_sw128(smem_u32(sB + stage * Cfg::kBBytes));
                 wgmma_fence();
                 fence_regs(acc);
+                uint32_t nk = kBK / 16;
+                if constexpr (KT) {                       // k-steps of this chunk that hold data: a source's last chunk may be short
+                    const uint32_t kx = jc < p.kc1 ? p.k1 - jc * kBK : p.k2 - (jc - p.kc1) * kBK;
+                    nk = kx >= (uint32_t)kBK ? kBK / 16 : (kx + 15u) / 16u;
+                    if (++jc == p.kc1 + p.kc2) jc = 0;
+                }
 #pragma unroll
                 for (uint32_t k = 0; k < kBK / 16; ++k) {   // advance 16 halves = 32 B = 2 descriptor units along K
+                    if (KT && k >= nk) break;
                     if constexpr (BN == 256) wgmma_ss_n256(acc, a_desc + 2 * k, b_desc + 2 * k, 1u);
                     else if constexpr (BN == 128) wgmma_ss_n128(acc, a_desc + 2 * k, b_desc + 2 * k, 1u);
+                    else if constexpr (BN == 160) wgmma_ss_n160(acc, a_desc + 2 * k, b_desc + 2 * k, 1u);
+                    else if constexpr (BN == 80) wgmma_ss_n80(acc, a_desc + 2 * k, b_desc + 2 * k, 1u);
+                    else if constexpr (BN == 48) wgmma_ss_n48(acc, a_desc + 2 * k, b_desc + 2 * k, 1u);
+                    else if constexpr (BN == 40) wgmma_ss_n40(acc, a_desc + 2 * k, b_desc + 2 * k, 1u);
+                    else if constexpr (BN == 16) wgmma_ss_n16(acc, a_desc + 2 * k, b_desc + 2 * k, 1u);
                     else wgmma_ss_n64(acc, a_desc + 2 * k, b_desc + 2 * k, 1u);
                 }
                 wgmma_commit();
@@ -309,13 +330,13 @@ int make_map_4d_box(CUtensorMap* m, const void* base, uint64_t K, uint64_t e1, u
 }
 int conv_row2_launch(const ssdnerf_gemm_args* a, int sms, cudaStream_t stream);   // conv_row2.cu
 
-template <int BN, int CL>
+template <int BN, int CL, bool KT = false>
 static int launch_gemm(const CUtensorMap& mA1, const CUtensorMap& mA2, const CUtensorMap& mB, const GemmParams& p, int sms,
                        cudaStream_t stream) {
     using Cfg = GemmCfg<BN, CL>;
     static DeviceOnce attr;
     if (attr.first()) {
-        SSDNERF_CUDA_OK(cudaFuncSetAttribute(k_gemm_tc<BN, CL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::kSmem));
+        SSDNERF_CUDA_OK(cudaFuncSetAttribute(k_gemm_tc<BN, CL, KT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::kSmem));
     }
     const uint32_t tiles_m = p.T1 * p.T2 * p.T3;
     const uint32_t total = ((tiles_m + CL - 1) / CL) * p.tiles_n;          // work items per cluster (CL = 1: per CTA)
@@ -337,7 +358,7 @@ static int launch_gemm(const CUtensorMap& mA1, const CUtensorMap& mA2, const CUt
             cfg.gridDim = dim3((uint32_t)(sms / CL) * CL);
             int n = 0;
             cfg.numAttrs = 1;
-            if (cudaOccupancyMaxActiveClusters(&n, k_gemm_tc<BN, CL>, &cfg) == cudaSuccess && n > 0 && n < max_clusters_cached) max_clusters_cached = n;
+            if (cudaOccupancyMaxActiveClusters(&n, k_gemm_tc<BN, CL, KT>, &cfg) == cudaSuccess && n > 0 && n < max_clusters_cached) max_clusters_cached = n;
             cfg.numAttrs = 2;
             (void)cudaGetLastError();
         }
@@ -345,7 +366,7 @@ static int launch_gemm(const CUtensorMap& mA1, const CUtensorMap& mA2, const CUt
     const uint32_t max_clusters = (uint32_t)max_clusters_cached;
     const uint32_t clusters = total < max_clusters ? total : max_clusters;
     cfg.gridDim = dim3(clusters * CL);
-    SSDNERF_CUDA_OK(cudaLaunchKernelEx(&cfg, k_gemm_tc<BN, CL>, mA1, mA2, mB, p));
+    SSDNERF_CUDA_OK(cudaLaunchKernelEx(&cfg, k_gemm_tc<BN, CL, KT>, mA1, mA2, mB, p));
     SSDNERF_LAUNCH_OK();
     return 0;
 }
@@ -357,7 +378,15 @@ using namespace ssdnerf;
 extern "C" int ssdnerf_gemm_f16(const ssdnerf_gemm_args* a, void* stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
     if (!a || !a->a1 || !a->b || !a->out) return set_error_msg(SSDNERF_ERR_ARG, "gemm: a1, b and out are required");
-    if (a->k1 == 0 || a->k1 % 64 || a->k2 % 64) return set_error_msg(SSDNERF_ERR_ARG, "gemm: K extents must be multiples of 64");
+    // algo 3 = narrow-channel family: K extents multiples of 8 (16-byte TMA rows), N tiles fitted to N (see the header comment)
+    const bool kt = a->algo == 3;
+    if (kt) {
+        if (a->k1 == 0 || a->k1 % 8 || (a->a2 && (a->k2 == 0 || a->k2 % 8)))
+            return set_error_msg(SSDNERF_ERR_ARG, "gemm (narrow): K extents must be multiples of 8");
+        if (a->cluster > 1) return set_error_msg(SSDNERF_ERR_ARG, "gemm (narrow): clusters are not built");
+    } else if (a->k1 == 0 || a->k1 % 64 || a->k2 % 64) {
+        return set_error_msg(SSDNERF_ERR_ARG, "gemm: K extents must be multiples of 64");
+    }
     if (a->b1 * a->b2 * a->b3 != 128) return set_error_msg(SSDNERF_ERR_ARG, "gemm: b1*b2*b3 must be 128");
     if (a->taps < 1 || a->taps > 9) return set_error_msg(SSDNERF_ERR_ARG, "gemm: taps must be in [1, 9]");
     if (a->taps != 1 && a->taps != 9 && !a->tap_offsets) return set_error_msg(SSDNERF_ERR_ARG, "gemm: taps other than 1 / 9 need tap_offsets");
@@ -370,13 +399,27 @@ extern "C" int ssdnerf_gemm_f16(const ssdnerf_gemm_args* a, void* stream_) {
     SSDNERF_CUDA_OK(cudaGetDevice(&dev));
     SSDNERF_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     // 3x3 convolution over 128-pixel rows with 128 output channels (the UNet's 128 x 128 level): row-pair kernel with halo reuse
-    if (a->algo != 1 && a->taps == 9 && !a->tap_offsets && a_stride == 1 && a->d1 == 128 && a->b1 == 128 && a->b2 == 1 && a->b3 == 1 && a->n == 128 && !a->out_f32 && !a->b_batched &&
+    if (a->algo != 1 && !kt && a->taps == 9 && !a->tap_offsets && a_stride == 1 && a->d1 == 128 && a->b1 == 128 && a->b2 == 1 && a->b3 == 1 && a->n == 128 && !a->out_f32 && !a->b_batched &&
         (a->d2 % 2) == 0 && a->alpha == 1.0f && (a->bn == 0 || a->bn == 128) && a->cluster <= 1 && a->so1 == 128 && a->so2 == 128 * 128 &&
         a->so3 == (long long)a->d2 * 128 * 128 && (!a->qstats || a->stats_hw == 0) && (a->n_rows_b == 0 || a->n_rows_b >= 128))
         return ssdnerf::conv_row2_launch(a, sms, stream);
     if (a->algo == 2) return set_error_msg(SSDNERF_ERR_ARG, "gemm: algo 2 (row-pair convolution) needs taps 9, 128-pixel rows, 128 output channels, fp16 output");
     int bn = (int)a->bn;
-    if (!bn) {
+    if (kt) {
+        // the largest tile that divides N; otherwise the one that computes the fewest padding columns (ties: the wider tile)
+        const int cand[6] = {256, 160, 80, 48, 40, 16};
+        if (bn) {
+            bool ok = false;
+            for (int c : cand) ok |= c == bn;
+            if (!ok) return set_error_msg(SSDNERF_ERR_ARG, "gemm (narrow): bn must be 16, 40, 48, 80, 160 or 256");
+        } else {
+            for (int c : cand) if (a->n % (uint32_t)c == 0) { bn = c; break; }
+            if (!bn) {
+                uint32_t best = 0xFFFFFFFFu;
+                for (int c : cand) { const uint32_t w = div_up(a->n, (uint32_t)c) * (uint32_t)c; if (w < best) { best = w; bn = c; } }
+            }
+        }
+    } else if (!bn) {
         // pick the N tile that minimises (waves x tile cost): wide tiles amortise A loads (a 64 x 256 wgmma per consumer warpgroup
         // keeps the tensor cores busiest, N=128 and N=64 re-read A more often) but small problems need more tiles to fill every SM
         const uint32_t tiles_m = div_up(a->d1, a->b1) * div_up(a->d2, a->b2) * div_up(a->d3, a->b3);
@@ -390,7 +433,7 @@ extern "C" int ssdnerf_gemm_f16(const ssdnerf_gemm_args* a, void* stream_) {
             if (t < best) { best = t; bn = cand[i]; }
         }
     }
-    if (bn != 64 && bn != 128 && bn != 256) return set_error_msg(SSDNERF_ERR_ARG, "gemm: bn must be 64, 128 or 256");
+    if (!kt && bn != 64 && bn != 128 && bn != 256) return set_error_msg(SSDNERF_ERR_ARG, "gemm: bn must be 64, 128 or 256");
 
     GemmParams p{};
     p.b1 = a->b1; p.b2 = a->b2; p.b3 = a->b3; p.d1 = a->d1; p.d2 = a->d2; p.d3 = a->d3;
@@ -402,7 +445,8 @@ extern "C" int ssdnerf_gemm_f16(const ssdnerf_gemm_args* a, void* stream_) {
         else if (a->taps == 9) { p.tap_ox[t] = (int8_t)((int)(t % 3) - 1); p.tap_oy[t] = (int8_t)((int)(t / 3) - 1); }
         else { p.tap_ox[t] = 0; p.tap_oy[t] = 0; }
     }
-    p.taps = a->taps; p.kc1 = a->k1 / 64; p.kc2 = a->a2 ? a->k2 / 64 : 0; p.n_valid = a->n; p.b_batched = a->b_batched;
+    p.taps = a->taps; p.kc1 = div_up(a->k1, 64u); p.kc2 = a->a2 ? div_up(a->k2, 64u) : 0;
+    p.k1 = a->k1; p.k2 = a->a2 ? a->k2 : 0; p.n_valid = a->n; p.b_batched = a->b_batched;
     p.alpha = a->alpha; p.bias_n = a->bias_n; p.residual = (const __half*)a->residual; p.out = a->out; p.out_f32 = a->out_f32;
     p.so1 = a->so1; p.so2 = a->so2; p.so3 = a->so3;
     p.qstats = a->qstats; p.stats_hw = a->stats_hw; p.prof = (unsigned long long*)a->debug_cycles;
@@ -432,6 +476,16 @@ extern "C" int ssdnerf_gemm_f16(const ssdnerf_gemm_args* a, void* stream_) {
     if (int e = make_map_4d(&mB, a->b, ktot, a->n_rows_b ? a->n_rows_b : a->n, a->bx2 ? a->bx2 : 1, a->bx3 ? a->bx3 : 1, a->b_strides[0],
                             a->b_strides[1], a->b_strides[2], (uint32_t)(bn / cl), 1, 1)) return e;
 
+    if (kt) {
+        switch (bn) {
+            case 256: return launch_gemm<256, 1, true>(mA1, mA2, mB, p, sms, stream);
+            case 160: return launch_gemm<160, 1, true>(mA1, mA2, mB, p, sms, stream);
+            case 80: return launch_gemm<80, 1, true>(mA1, mA2, mB, p, sms, stream);
+            case 48: return launch_gemm<48, 1, true>(mA1, mA2, mB, p, sms, stream);
+            case 40: return launch_gemm<40, 1, true>(mA1, mA2, mB, p, sms, stream);
+            default: return launch_gemm<16, 1, true>(mA1, mA2, mB, p, sms, stream);
+        }
+    }
     if (bn == 256) {
         if (cl == 8) return launch_gemm<256, 8>(mA1, mA2, mB, p, sms, stream);
         if (cl == 4) return launch_gemm<256, 4>(mA1, mA2, mB, p, sms, stream);

@@ -368,7 +368,7 @@ class GaussianDiffusion(nn.Module):
             ts = self.ddim_timesteps(num_steps)
             lanes = []
             for i in range(n_lanes):
-                eng = unet.engine(Bl, dev) if i == 0 else UNetEngine(unet, Bl, dev)
+                eng = unet.engine(Bl, dev, (H, W)) if i == 0 else UNetEngine(unet, Bl, dev, (H, W))
                 lanes.append(dict(eng=eng, graph=None, lo=i * Bl, hi=(i + 1) * Bl,
                                   stream=torch.cuda.Stream(device=dev) if n_lanes > 1 else None,
                                   x_t=torch.empty(Bl, C, H, W, dtype=torch.float32, device=dev),

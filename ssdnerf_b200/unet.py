@@ -174,14 +174,16 @@ class DenoisingUnetMod(nn.Module):
         self._engine_key = None
 
     # ------------------------------------------------------------------ reference-facing API
-    def engine(self, batch, device=None):
-        """(re)build the native engine for a batch size; weights are re-packed when parameters changed"""
+    def engine(self, batch, device=None, hw=None):
+        """(re)build the native engine for a batch size and latent size hw = (H, W) (default: image_size); weights are re-packed when
+        parameters changed"""
         device = device or next(self.parameters()).device
-        key = (batch, str(device), tuple(p._version for p in self.parameters()))
+        hw = tuple(int(v) for v in (hw if hw is not None else self.image_size))
+        key = (batch, str(device), hw, tuple(p._version for p in self.parameters()))
         if self._engine is None or self._engine_key != key:
             old = self._engine
-            self._engine = UNetEngine(self, batch, device)
-            if old is not None and self._engine_key is not None and self._engine_key[:2] == key[:2]:
+            self._engine = UNetEngine(self, batch, device, hw)
+            if old is not None and self._engine_key is not None and self._engine_key[:3] == key[:3]:
                 self._engine.bufs = old.bufs          # only the weights changed (optimizer step): keep the activation / scratch arena
             self._engine_key = key
         return self._engine
@@ -221,7 +223,7 @@ class DenoisingUnetMod(nn.Module):
                 raise NotImplementedError('input gradients with concat_cond are not built (unused by the shipped configs)')
             return _UNetInputGrad.apply(h, self, t)
         with torch.no_grad():
-            eng = self.engine(B, h.device)
+            eng = self.engine(B, h.device, h.shape[-2:])
             eng.set_embedding(self.embedding(t.to(h.device)))
             v = eng.forward_nchw(h.float().contiguous())
             return v.permute(0, 3, 1, 2)[:, :self.out_channels].contiguous()
@@ -234,7 +236,7 @@ class _UNetInputGrad(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x_t, module, t):
         B = x_t.shape[0]
-        eng = module.engine(B, x_t.device)
+        eng = module.engine(B, x_t.device, x_t.shape[-2:])
         eng.set_embedding(module.embedding(t.to(x_t.device)))
         eng.load_input_nchw(x_t.detach().float().contiguous())
         v = eng.forward_nhwc(save=True)
@@ -249,26 +251,49 @@ class _UNetInputGrad(torch.autograd.Function):
         return eng.backward_nchw(grad_v.contiguous().float()), None, None
 
 
+def unet_widths(m):
+    return sorted({m.base_channels * f for f in m.channel_factor_list} | {m.base_channels})
+
+
+def is_narrow(m):
+    """widths that are not all multiples of 64 (the tiled-triplane config: 80 / 160 / 320) run on the narrow-channel GEMM family"""
+    return any(w % 64 for w in unet_widths(m))
+
+
 class UNetEngine:
-    """Packed fp16 weights + activation arena + launch sequence for one batch size."""
+    """Packed fp16 weights + activation arena + launch sequence for one batch size and latent size.
+
+    Channel widths must be multiples of 16 and divisible by the GroupNorm group count.  Widths that are all multiples of 64 (every
+    paper config) use the default GEMM family; otherwise (`narrow`: the tiled-triplane config's 80 / 160 / 320 channels, GroupNorm(16),
+    40 / 80-wide heads over 6 x 128 x 384 latents) every GEMM runs on the narrow-channel family (unet_ops, csrc/gemm_tc.cu algo 3),
+    attention takes the unfused composition, the input is padded to 16 channels instead of 64, and the weight-gradient pass is not
+    built (unet_train.WeightGradPass raises)."""
 
     CPAD_IN = 64
 
-    def __init__(self, m: DenoisingUnetMod, batch, device):
+    def __init__(self, m: DenoisingUnetMod, batch, device, hw=None):
         self.m, self.B, self.dev = m, batch, torch.device(device)
-        widths = sorted({m.base_channels * f for f in m.channel_factor_list} | {m.base_channels})
-        if m.num_groups != 32 or any(w % 64 for w in widths):
-            raise NotImplementedError(
-                f'native UNet engine: channel widths must be multiples of 64 with GroupNorm(32) (every paper config: base 128); got widths '
-                f'{widths}, {m.num_groups} groups (configs/new_cfgs/*_tiled.py builds and loads checkpoints but has no kernels yet)')
+        widths = unet_widths(m)
+        self.groups = m.num_groups
+        if any(w % 16 for w in widths) or any(w % self.groups for w in widths):
+            raise NotImplementedError(f'native UNet engine: channel widths must be multiples of 16 and of the GroupNorm group count; got '
+                                      f'widths {widths}, {self.groups} groups')
+        self.narrow = is_narrow(m)
+        attn_widths = sorted({p.c for p in m.modules() if isinstance(p, _AttnParams)})
+        if any(c % m.num_heads or (c // m.num_heads) % 8 for c in attn_widths):
+            raise NotImplementedError(f'native UNet engine: attention head widths must be multiples of 8; got widths {attn_widths} over '
+                                      f'{m.num_heads} heads')
         self.flash_attention = True      # False: unfused scores -> softmax -> PV composition (A/B tests)
         # 128x128-level resblocks: GroupNorm + SiLU inside the row-pair conv kernel (csrc/conv_row2.cu).  Opt-in (SSDNERF_FUSED_GN_CONV=1):
         # the default is the GroupNorm-apply pass followed by the row-pair convolution
         self.fused_gn_conv = os.environ.get('SSDNERF_FUSED_GN_CONV', '0') == '1'
-        self.H, self.W = m.image_size
+        self.H, self.W = (int(v) for v in (hw if hw is not None else m.image_size))
         self.bufs = {}
         self.cin_total = m.in_channels + m.concat_cond_channels
+        if self.narrow:       # the input convolution's K: the channels rounded up to wgmma's 16-element K step, not to 64
+            self.CPAD_IN = max(16, (self.cin_total + 15) // 16 * 16)
         assert self.cin_total <= self.CPAD_IN
+        nw = self.narrow
         dev = self.dev
         f32 = lambda p: p.detach().float().contiguous().to(dev)
         # ---- op list + packed weights
@@ -278,29 +303,30 @@ class UNetEngine:
 
         def res(p):
             d = dict(cin=p.cin, cout=p.cout, g1=f32(p.conv_1[0].weight), b1=f32(p.conv_1[0].bias),
-                     w1=U.pack_conv_weight(p.conv_1[2].weight).to(dev), c1b=f32(p.conv_1[2].bias),
+                     w1=U.pack_conv_weight(p.conv_1[2].weight, narrow=nw).to(dev), c1b=f32(p.conv_1[2].bias),
                      g2=f32(p.norm_with_embedding.norm.weight), b2=f32(p.norm_with_embedding.norm.bias),
-                     w2=U.pack_conv_weight(p.conv_2[-1].weight).to(dev), c2b=f32(p.conv_2[-1].bias),
+                     w2=U.pack_conv_weight(p.conv_2[-1].weight, narrow=nw).to(dev), c2b=f32(p.conv_2[-1].bias),
                      emb_w=f32(p.norm_with_embedding.embedding_layer[1].weight), emb_b=f32(p.norm_with_embedding.embedding_layer[1].bias),
                      n1=self._norm_slot(), n2=self._norm_slot(), idx=len(self.res_blocks), mod=p)
             if hasattr(p, 'shortcut'):
-                d['ws'] = U.pack_linear_weight(p.shortcut.weight).to(dev)
+                d['ws'] = U.pack_linear_weight(p.shortcut.weight, narrow=nw).to(dev)
                 d['wsb'] = f32(p.shortcut.bias)
             self.res_blocks.append(d)
             return ('res', d)
 
         def attn(p):
             return ('attn', dict(c=p.c, heads=p.num_heads, g=f32(p.norm.weight), b=f32(p.norm.bias),
-                                 wqkv=U.pack_linear_weight(p.qkv.weight).to(dev), bqkv=f32(p.qkv.bias),
-                                 wproj=U.pack_linear_weight(p.proj.weight).to(dev), bproj=f32(p.proj.bias), n=self._norm_slot(), mod=p))
+                                 wqkv=U.pack_linear_weight(p.qkv.weight, narrow=nw).to(dev), bqkv=f32(p.qkv.bias),
+                                 wproj=U.pack_linear_weight(p.proj.weight, narrow=nw).to(dev), bproj=f32(p.proj.bias), n=self._norm_slot(),
+                                 mod=p))
 
         def layer(p):
             if isinstance(p, _ResBlockParams): return res(p)
             if isinstance(p, _AttnParams): return attn(p)
             if isinstance(p, _DownParams):
-                return ('down', dict(c=p.c, w=U.pack_conv_weight(p.downsample.weight).to(dev), b=f32(p.downsample.bias), mod=p))
+                return ('down', dict(c=p.c, w=U.pack_conv_weight(p.downsample.weight, narrow=nw).to(dev), b=f32(p.downsample.bias), mod=p))
             if isinstance(p, _UpParams):
-                return ('up', dict(c=p.c, w=U.pack_upconv_weight(p.conv.weight).to(dev), b=f32(p.conv.bias), mod=p))
+                return ('up', dict(c=p.c, w=U.pack_upconv_weight(p.conv.weight, narrow=nw).to(dev), b=f32(p.conv.bias), mod=p))
             raise TypeError(type(p))
 
         conv_in = m.in_blocks[0][0]
@@ -309,7 +335,7 @@ class UNetEngine:
         self.mid_seq = [layer(p) for p in m.mid_blocks]
         self.out_seq = [[layer(p) for p in blk] for blk in m.out_blocks]
         self.out_norm = dict(g=f32(m.out.gn.weight), b=f32(m.out.gn.bias), n=self._norm_slot(), c=m.out.gn.num_channels)
-        self.out_conv = dict(w=U.pack_conv_weight(m.out.conv.weight).to(dev), b=f32(m.out.conv.bias), cout=m.out.conv.out_channels)
+        self.out_conv = dict(w=U.pack_conv_weight(m.out.conv.weight, narrow=nw).to(dev), b=f32(m.out.conv.bias), cout=m.out.conv.out_channels)
         # ---- GroupNorm quad-statistics arena: one [B, C/4, 2] slice per tensor that feeds a norm, filled by the producing GEMM's
         #      epilogue; zeroed once per forward (a single memset node in the captured graph)
         self.qarena = torch.zeros(4 * 1024 * 1024, dtype=torch.float32, device=dev)
@@ -362,7 +388,11 @@ class UNetEngine:
 
     # ------------------------------------------------------------------ kernels
     def _q(self, key, channels):
-        """quad-statistics slice [B, C/4, 2] for the tensor produced at `key` (stable across forwards: graph-capturable)"""
+        """quad-statistics slice [B, C/4, 2] for the tensor produced at `key` (stable across forwards: graph-capturable); None where a
+        GroupNorm group of this tensor is not a whole number of quads (GroupNorm(16) over 80 / 160 channels): its producer then emits
+        no statistics and the norm takes the separate statistics pass"""
+        if (channels // self.groups) % 4:
+            return None
         t = self.qslots.get(key)
         if t is None:
             n = self.B * (channels // 4) * 2
@@ -373,26 +403,28 @@ class UNetEngine:
         return t
 
     def _gn(self, x1, q1, x2, q2, gamma, beta, out, silu, ss_off=None):
-        """GroupNorm(32) over the channel concat of x1 (+x2) from the quad statistics their producers emitted.
+        """GroupNorm(self.groups) over the channel concat of x1 (+x2) from the quad statistics their producers emitted.
         Leaves the statistics descriptor the backward needs in `self._last_stats` = (is_quad, stats1, stats2)."""
         B, H, W, C1 = x1.shape
         C2 = x2.shape[-1] if x2 is not None else 0
+        G = self.groups
         L, s = N.lib(), N.stream_ptr()
         ss = None
         if ss_off is not None:
             ss = N.c_void_p(self.ss_cur.data_ptr() + 4 * ss_off)
-        if ((C1 + C2) // 32) % 4 != 0:
-            # fewer than 4 channels per group (only sub-128-channel toy configs): separate statistics pass over group sums
+        if ((C1 + C2) // G) % 4 != 0 or q1 is None or (x2 is not None and q2 is None):
+            # a group is not a whole number of 4-channel quads (sub-128-channel toy configs; GroupNorm(16) over 80 / 160 / 240 / 480
+            # channels), or the producer could not emit quad statistics: separate statistics pass over group sums
             self._legacy_idx += 1          # one slot per call site, in call order (stable across forwards)
-            st = self._q(('legacy', self._legacy_idx), 32 * 4)     # [B, 32, 2], contiguous
-            N.check(L.ssdnerf_gn_stats(N.ptr(x1), N.c_u32(C1), N.ptr(x2), N.c_u32(C2), N.c_u32(B), N.c_u32(H * W), N.c_u32(32), N.ptr(st), s))
-            N.check(L.ssdnerf_gn_apply(N.ptr(x1), N.c_u32(C1), N.ptr(x2), N.c_u32(C2), N.c_u32(B), N.c_u32(H * W), N.c_u32(32), N.ptr(st),
+            st = self._q(('legacy', self._legacy_idx), G * 4)      # [B, G, 2], contiguous
+            N.check(L.ssdnerf_gn_stats(N.ptr(x1), N.c_u32(C1), N.ptr(x2), N.c_u32(C2), N.c_u32(B), N.c_u32(H * W), N.c_u32(G), N.ptr(st), s))
+            N.check(L.ssdnerf_gn_apply(N.ptr(x1), N.c_u32(C1), N.ptr(x2), N.c_u32(C2), N.c_u32(B), N.c_u32(H * W), N.c_u32(G), N.ptr(st),
                                        N.ptr(gamma), N.ptr(beta), ss, N.c_longlong(self.ss_total), N.c_f32(1e-5), N.c_int(int(silu)),
                                        N.ptr(out), s))
             self._last_stats = (False, st, None)
             return out
         self._last_stats = (True, q1, q2)
-        N.check(L.ssdnerf_gn_apply_q(N.ptr(x1), N.c_u32(C1), N.ptr(x2), N.c_u32(C2), N.c_u32(B), N.c_u32(H * W), N.c_u32(32), N.ptr(q1),
+        N.check(L.ssdnerf_gn_apply_q(N.ptr(x1), N.c_u32(C1), N.ptr(x2), N.c_u32(C2), N.c_u32(B), N.c_u32(H * W), N.c_u32(G), N.ptr(q1),
                                      N.ptr(q2), N.ptr(gamma), N.ptr(beta), ss, N.c_longlong(self.ss_total), N.c_f32(1e-5),
                                      N.c_int(int(silu)), N.ptr(out), s))
         return out
@@ -402,8 +434,10 @@ class UNetEngine:
         (x, qx), (sk, qs) = x, (skip if skip is not None else (None, None))
         B, H, W, _ = x.shape
         cin, cout = d['cin'], d['cout']
+        nw = self.narrow
         if 'ws' in d:
-            sc = U.conv3x3_f16(x, d['ws'].unsqueeze(0), cout, bias=d['wsb'], x2=sk, taps=1, out=self._buf(('sc', H, cout), (B, H, W, cout)))
+            sc = U.conv3x3_f16(x, d['ws'].unsqueeze(0), cout, bias=d['wsb'], x2=sk, taps=1, out=self._buf(('sc', H, cout), (B, H, W, cout)),
+                               narrow=nw)
         else:
             if sk is not None:      # an identity shortcut over a channel concat would need the concatenated tensor (mmgen adds it whole);
                 raise NotImplementedError('ResBlock with a skip concat but no shortcut convolution (cin + skip == cout) is not built')
@@ -413,14 +447,15 @@ class UNetEngine:
         if self.saving:       # keep what the input-gradient pass re-reads: raw inputs of both GroupNorms + their statistics
             a = self._gn(x, qx, sk, qs, d['g1'], d['b1'], self._buf(('a', H, cin), (B, H, W, cin)), True)
             st1 = self._last_stats
-            h1 = U.conv3x3_f16(a, d['w1'], cout, bias=d['c1b'], out=self._buf(('h1', tag), (B, H, W, cout)), qstats=qh1)
+            h1 = U.conv3x3_f16(a, d['w1'], cout, bias=d['c1b'], out=self._buf(('h1', tag), (B, H, W, cout)), qstats=qh1, narrow=nw)
             a2 = self._gn(h1, qh1, None, None, d['g2'], d['b2'], self._buf(('a2', H, cout), (B, H, W, cout)), True, self.ss_offsets[d['idx']])
             st2 = self._last_stats
             self._dropout(a2, d['idx'])
-            out = U.conv3x3_f16(a2, d['w2'], cout, bias=d['c2b'], residual=sc, out=self._buf(('res_out', tag), (B, H, W, cout)), qstats=qo)
+            out = U.conv3x3_f16(a2, d['w2'], cout, bias=d['c2b'], residual=sc, out=self._buf(('res_out', tag), (B, H, W, cout)), qstats=qo,
+                                narrow=nw)
             self.tape.append(dict(kind='res', d=d, x=x, sk=sk, st1=st1, h1=h1, st2=st2, out=out, tag=tag))
             return out, qo
-        if self.fused_gn_conv and W == 128 and cout == 128 and cin <= 384 and (cin // 32) % 4 == 0:
+        if self.fused_gn_conv and not nw and self.groups == 32 and W == 128 and cout == 128 and cin <= 384 and (cin // 32) % 4 == 0:
             # 128 x 128 level: GroupNorm apply + SiLU ride on the convolution's activation load path (csrc/conv_row2_gn.cu)
             h1 = U.conv3x3_gn_f16(x, qx, d['g1'], d['b1'], d['w1'], bias=d['c1b'], x2=sk, q2=qs,
                                   out=self._buf(('h1', H, cout), (B, H, W, cout)), qstats=qh1,
@@ -430,9 +465,10 @@ class UNetEngine:
                                     residual=sc, out=self._buf(('res_out', tag), (B, H, W, cout)), qstats=qo,
                                     coef_ws=self._buf(('gncoef', 2, tag), (B * cout * 2,), torch.float32)), qo
         a = self._gn(x, qx, sk, qs, d['g1'], d['b1'], self._buf(('a', H, cin), (B, H, W, cin)), True)
-        h1 = U.conv3x3_f16(a, d['w1'], cout, bias=d['c1b'], out=self._buf(('h1', H, cout), (B, H, W, cout)), qstats=qh1)
+        h1 = U.conv3x3_f16(a, d['w1'], cout, bias=d['c1b'], out=self._buf(('h1', H, cout), (B, H, W, cout)), qstats=qh1, narrow=nw)
         a2 = self._gn(h1, qh1, None, None, d['g2'], d['b2'], self._buf(('a2', H, cout), (B, H, W, cout)), True, self.ss_offsets[d['idx']])
-        return U.conv3x3_f16(a2, d['w2'], cout, bias=d['c2b'], residual=sc, out=self._buf(('res_out', tag), (B, H, W, cout)), qstats=qo), qo
+        return U.conv3x3_f16(a2, d['w2'], cout, bias=d['c2b'], residual=sc, out=self._buf(('res_out', tag), (B, H, W, cout)), qstats=qo,
+                             narrow=nw), qo
 
     def _attn(self, d, x, tag):
         x, qx = x
@@ -443,11 +479,13 @@ class UNetEngine:
         xn = self._gn(x, qx, None, None, d['g'], d['b'], self._buf(('xn', T, c), (B, H, W, c)), False)
         st = self._last_stats
         qkv = U.linear_f16(xn.view(B * T, c), d['wqkv'], bias=d['bqkv'], n=3 * c,
-                           out=self._buf(('qkv', tag) if self.saving else ('qkv', T, c), (B * T, 3 * c)))
+                           out=self._buf(('qkv', tag) if self.saving else ('qkv', T, c), (B * T, 3 * c)), narrow=self.narrow)
         o = self._attn_core(qkv, B, T, c, heads, ('o', T, c))
-        qo = self._q(('attn_out', tag), c)
+        # the projection's epilogue emits per-image quad statistics when an image is a whole number of 64-row tile halves; otherwise
+        # (T = 48 at the tiled config's 4 x 12 level) the next GroupNorm takes the separate statistics pass
+        qo = self._q(('attn_out', tag), c) if T % 64 == 0 else None
         out = U.linear_f16(o.view(B * T, c), d['wproj'], bias=d['bproj'], residual=x.view(B * T, c), n=c,
-                           out=self._buf(('attn_out', tag), (B * T, c)), qstats=qo, stats_hw=T).view(B, H, W, c)
+                           out=self._buf(('attn_out', tag), (B * T, c)), qstats=qo, stats_hw=T, narrow=self.narrow).view(B, H, W, c)
         if self.saving:
             self.tape.append(dict(kind='attn', d=d, x=x, st=st, qkv=qkv.view(B, T, 3 * c), out=out, tag=tag))
         return out, qo
@@ -459,19 +497,20 @@ class UNetEngine:
         if self.flash_attention and ch in (64, 128) and T % 64 == 0:
             return U.flash_attn(qkv.view(B, T, 3 * c), heads, 1.0 / math.sqrt(ch), out=self._buf(out_key, (B, T, c)))
         # unfused composition (scores -> softmax -> P V), kept for head widths / lengths the fused kernel does not cover
-        S = U.attn_scores(qkv.view(B, T, 3 * c), heads, scale=1.0 / math.sqrt(ch), out=self._buf(('S', T), (B, heads, T, T), torch.float32))
+        S = U.attn_scores(qkv.view(B, T, 3 * c), heads, scale=1.0 / math.sqrt(ch), out=self._buf(('S', T), (B, heads, T, T), torch.float32),
+                          narrow=self.narrow)
         P = self._buf(('P', T), (B, heads, T, T))
         N.check(L.ssdnerf_softmax_rows(N.ptr(S), N.c_u32(B * heads * T), N.c_u32(T), N.ptr(P), s))
         vt = self._buf(('vt', T, c), (B, heads, ch, T))
         N.check(L.ssdnerf_transpose_v(N.ptr(qkv), N.c_u32(B), N.c_u32(T), N.c_u32(heads), N.c_u32(ch), N.ptr(vt), s))
-        return U.attn_pv(P, vt, out=self._buf(out_key, (B, T, c)))
+        return U.attn_pv(P, vt, out=self._buf(out_key, (B, T, c)), narrow=self.narrow)
 
     def _down(self, d, x, tag):
         x, _ = x
         B, H, W, c = x.shape
         qo = self._q(('down_out', tag), c)
         # stride-2 convolution straight from x: TMA boxes traverse every second pixel (no im2col buffer)
-        out = U.conv3x3_s2_f16(x, d['w'], c, bias=d['b'], out=self._buf(('down_out', tag), (B, H // 2, W // 2, c)), qstats=qo)
+        out = U.conv3x3_s2_f16(x, d['w'], c, bias=d['b'], out=self._buf(('down_out', tag), (B, H // 2, W // 2, c)), qstats=qo, narrow=self.narrow)
         if self.saving:
             self.tape.append(dict(kind='down', d=d, x=x, out=out, tag=tag))
         return out, qo
@@ -481,7 +520,7 @@ class UNetEngine:
         B, H, W, c = x.shape
         qo = self._q(('up_out', tag), c)
         # nearest x2 + conv3x3 as four 2x2-tap phase convolutions of the low-resolution tensor (no upsampled buffer, 4/9 of the flops)
-        out = U.upconv3x3_f16(x, d['w'], c, bias=d['b'], out=self._buf(('up_out', tag), (B, 2 * H, 2 * W, c)), qstats=qo)
+        out = U.upconv3x3_f16(x, d['w'], c, bias=d['b'], out=self._buf(('up_out', tag), (B, 2 * H, 2 * W, c)), qstats=qo, narrow=self.narrow)
         if self.saving:
             self.tape.append(dict(kind='up', d=d, x=x, out=out, tag=tag))
         return out, qo
@@ -510,7 +549,7 @@ class UNetEngine:
         self._legacy_idx = 0
         q0 = self._q(('conv_in',), self.conv_in['cout'])
         h = (U.conv3x3_f16(self.x_in, self.conv_in['w'], self.conv_in['cout'], bias=self.conv_in['b'],
-                           out=self._buf(('conv_in',), (self.B, self.H, self.W, self.conv_in['cout'])), qstats=q0), q0)
+                           out=self._buf(('conv_in',), (self.B, self.H, self.W, self.conv_in['cout'])), qstats=q0, narrow=self.narrow), q0)
         if self.saving:
             self.tape.append(dict(kind='conv_in', out=h[0]))
         hs = [h]
@@ -525,37 +564,37 @@ class UNetEngine:
         a = self._gn(h, qh, None, None, self.out_norm['g'], self.out_norm['b'], self._buf(('a', H, c), (B, H, W, c)), True)
         if self.saving:
             self.tape.append(dict(kind='out', x=h, st=self._last_stats))
-        U.conv3x3_f16(a, self.out_conv['w'], self.out_conv['cout'], bias=self.out_conv['b'], out=self.v_out)
+        U.conv3x3_f16(a, self.out_conv['w'], self.out_conv['cout'], bias=self.out_conv['b'], out=self.v_out, narrow=self.narrow)
         self.saving = False
         return self.v_out
 
     # ------------------------------------------------------------------ input-gradient pass (+ weight-gradient hooks: unet_train.py)
     def _pack_backward_weights(self):
         """transposed / tap-flipped fp16 copies of every weight, packed on first use (guidance and val_optim only)"""
-        m, dev = self.m, self.dev
+        m, dev, nw = self.m, self.dev, self.narrow
 
         def params(seq, mods):
             for (kind, d), p in zip(seq, mods):
                 if kind == 'res':
-                    d['w1T'] = U.pack_conv_weight_dgrad(p.conv_1[2].weight).to(dev)
-                    d['w2T'] = U.pack_conv_weight_dgrad(p.conv_2[-1].weight).to(dev)
+                    d['w1T'] = U.pack_conv_weight_dgrad(p.conv_1[2].weight, narrow=nw).to(dev)
+                    d['w2T'] = U.pack_conv_weight_dgrad(p.conv_2[-1].weight, narrow=nw).to(dev)
                     if hasattr(p, 'shortcut'):
-                        d['wsT'] = U.pack_linear_weight_dgrad(p.shortcut.weight).to(dev)
+                        d['wsT'] = U.pack_linear_weight_dgrad(p.shortcut.weight, narrow=nw).to(dev)
                 elif kind == 'attn':
-                    d['wqkvT'] = U.pack_linear_weight_dgrad(p.qkv.weight).to(dev)
-                    d['wprojT'] = U.pack_linear_weight_dgrad(p.proj.weight).to(dev)
+                    d['wqkvT'] = U.pack_linear_weight_dgrad(p.qkv.weight, narrow=nw).to(dev)
+                    d['wprojT'] = U.pack_linear_weight_dgrad(p.proj.weight, narrow=nw).to(dev)
                 elif kind == 'down':
                     w = p.downsample.weight.detach().permute(0, 2, 3, 1).reshape(p.c, 9 * p.c)       # [c, tap*c + cin]
-                    d['wT'] = U.pack_linear_weight_dgrad(w).to(dev)
+                    d['wT'] = U.pack_linear_weight_dgrad(w, narrow=nw).to(dev)
                 elif kind == 'up':
-                    d['wT'] = U.pack_conv_weight_dgrad(p.conv.weight).to(dev)
+                    d['wT'] = U.pack_conv_weight_dgrad(p.conv.weight, narrow=nw).to(dev)
 
         for seq, blk in zip(self.in_seq, list(m.in_blocks)[1:]):
             params(seq, blk)
         params(self.mid_seq, m.mid_blocks)
         for seq, blk in zip(self.out_seq, m.out_blocks):
             params(seq, blk)
-        self.conv_in['wT'] = U.pack_conv_weight_dgrad(m.in_blocks[0][0].weight).to(dev)                 # K = 128, rows = cin (padded to 64)
+        self.conv_in['wT'] = U.pack_conv_weight_dgrad(m.in_blocks[0][0].weight, narrow=nw).to(dev)      # K = base width, rows = cin
         self.out_conv['wT'] = U.pack_conv_weight_dgrad(m.out.conv.weight, cout_pad=self.CPAD_IN).to(dev)  # K = 18 -> 64, rows = 128
         self._bwd_packed = True
 
@@ -587,6 +626,7 @@ class UNetEngine:
         if not self._bwd_packed:
             self._pack_backward_weights()
         L, s = N.lib(), N.stream_ptr
+        nw, G = self.narrow, self.groups
         grads = {}
 
         def gb(name, idx, shape, dtype=torch.float16):
@@ -608,10 +648,10 @@ class UNetEngine:
             if kind == 'out':
                 x = r['x']
                 B, H, W, c = x.shape
-                d_a = U.conv3x3_f16(g_v, self.out_conv['wT'], c, out=gb('d_a', (H, c), (B, H, W, c)))
+                d_a = U.conv3x3_f16(g_v, self.out_conv['wT'], c, out=gb('d_a', (H, c), (B, H, W, c)), narrow=nw)
                 dh = gb('dx', idx, (B, H, W, c))
                 cs = wg.csum(c) if wg else None
-                U.gn_bwd(x, None, r['st'], self.out_norm['g'], self.out_norm['b'], d_a, dh, silu=True, gsum=gsum, csum=cs)
+                U.gn_bwd(x, None, r['st'], self.out_norm['g'], self.out_norm['b'], d_a, dh, silu=True, gsum=gsum, csum=cs, groups=G)
                 if wg:
                     wg.out(r, g_v, cs)
                 acc(x, dh)
@@ -621,25 +661,25 @@ class UNetEngine:
                 B, H, W, C1 = x.shape
                 C2 = sk.shape[-1] if sk is not None else 0
                 cin, cout = d['cin'], d['cout']
-                d_a2 = U.conv3x3_f16(g, d['w2T'], cout, out=gb('d_a2', (H, cout), (B, H, W, cout)))
+                d_a2 = U.conv3x3_f16(g, d['w2T'], cout, out=gb('d_a2', (H, cout), (B, H, W, cout)), narrow=nw)
                 self._dropout(d_a2, d['idx'])                     # same mask as the forward (a no-op outside training)
                 d_h1 = gb('d_h1', (H, cout), (B, H, W, cout))
                 ss = N.c_void_p(self.ss_cur.data_ptr() + 4 * self.ss_offsets[d['idx']])
                 cs2 = wg.csum(cout) if wg else None
                 U.gn_bwd(h1, None, r['st2'], d['g2'], d['b2'], d_a2, d_h1, scale_shift_ptr=ss, ss_batch_stride=self.ss_total, silu=True, gsum=gsum,
-                         csum=cs2)
+                         csum=cs2, groups=G)
                 if wg:      # conv_2 / norm 2 / embedding rows now: cs2 and the 'a' scratch are reused below
                     wg.res_second(r, g, cs2)
-                d_a = U.conv3x3_f16(d_h1, d['w1T'], cin, out=gb('d_a', (H, cin), (B, H, W, cin)))
+                d_a = U.conv3x3_f16(d_h1, d['w1T'], cin, out=gb('d_a', (H, cin), (B, H, W, cin)), narrow=nw)
                 if 'wsT' in d:
-                    add = U.conv3x3_f16(g, d['wsT'].unsqueeze(0), cin, taps=1, out=gb('d_sc', (H, cin), (B, H, W, cin)))
+                    add = U.conv3x3_f16(g, d['wsT'].unsqueeze(0), cin, taps=1, out=gb('d_sc', (H, cin), (B, H, W, cin)), narrow=nw)
                 else:
                     assert sk is None and cin == cout
                     add = g
                 dx = gb('dx', idx, (B, H, W, C1))
                 dsk = gb('dsk', idx, (B, H, W, C2)) if sk is not None else None
                 cs1 = wg.csum(cin) if wg else None
-                U.gn_bwd(x, sk, r['st1'], d['g1'], d['b1'], d_a, dx, dsk, add=add, silu=True, gsum=gsum, csum=cs1)
+                U.gn_bwd(x, sk, r['st1'], d['g1'], d['b1'], d_a, dx, dsk, add=add, silu=True, gsum=gsum, csum=cs1, groups=G)
                 if wg:
                     wg.res_first(r, g, d_h1, cs1)
                 acc(x, dx)
@@ -650,13 +690,13 @@ class UNetEngine:
                 g = grads.pop(out.data_ptr())
                 B, H, W, c = x.shape
                 T, heads = H * W, d['heads']
-                d_o = U.linear_f16(g.view(B * T, c), d['wprojT'], n=c, out=gb('d_o', (T, c), (B * T, c)))
+                d_o = U.linear_f16(g.view(B * T, c), d['wprojT'], n=c, out=gb('d_o', (T, c), (B * T, c)), narrow=nw)
                 dqkv = U.attn_backward(qkv, d_o.view(B, T, c), heads, 1.0 / math.sqrt(c // heads),
-                                       lambda name, shape, dtype: gb('att_' + name, (T, c), shape, dtype))
-                d_xn = U.linear_f16(dqkv.view(B * T, 3 * c), d['wqkvT'], n=c, out=gb('d_xn', (T, c), (B * T, c)))
+                                       lambda name, shape, dtype: gb('att_' + name, (T, c), shape, dtype), narrow=nw)
+                d_xn = U.linear_f16(dqkv.view(B * T, 3 * c), d['wqkvT'], n=c, out=gb('d_xn', (T, c), (B * T, c)), narrow=nw)
                 dx = gb('dx', idx, (B, H, W, c))
                 cs = wg.csum(c) if wg else None
-                U.gn_bwd(x, None, r['st'], d['g'], d['b'], d_xn.view(B, H, W, c), dx, add=g, silu=False, gsum=gsum, csum=cs)
+                U.gn_bwd(x, None, r['st'], d['g'], d['b'], d_xn.view(B, H, W, c), dx, add=g, silu=False, gsum=gsum, csum=cs, groups=G)
                 if wg:
                     wg.attn(r, g, dqkv, cs)
                 acc(x, dx)
@@ -667,7 +707,7 @@ class UNetEngine:
                 if wg:
                     wg.down(r, g)
                 M = B * (H // 2) * (W // 2)
-                dcol = U.linear_f16(g.view(M, c), d['wT'], n=9 * c, out=gb('dcol', (H, c), (M, 9 * c)))
+                dcol = U.linear_f16(g.view(M, c), d['wT'], n=9 * c, out=gb('dcol', (H, c), (M, 9 * c)), narrow=nw)
                 dx = gb('dx', idx, (B, H, W, c))
                 old = grads.pop(x.data_ptr(), None)
                 N.check(L.ssdnerf_col2im_s2(N.ptr(dcol), N.c_u32(B), N.c_u32(H), N.c_u32(W), N.c_u32(c), N.ptr(old), N.ptr(dx), s()))
@@ -678,7 +718,7 @@ class UNetEngine:
                 B, H, W, c = x.shape
                 if wg:
                     wg.up(r, g)
-                dup = U.conv3x3_f16(g, d['wT'], c, out=gb('dup', (H, c), (B, 2 * H, 2 * W, c)))
+                dup = U.conv3x3_f16(g, d['wT'], c, out=gb('dup', (H, c), (B, 2 * H, 2 * W, c)), narrow=nw)
                 dx = gb('dx', idx, (B, H, W, c))
                 N.check(L.ssdnerf_sum2x2(N.ptr(dup), N.c_u32(B), N.c_u32(H), N.c_u32(W), N.c_u32(c), N.ptr(dx), s()))
                 acc(x, dx)
@@ -687,7 +727,7 @@ class UNetEngine:
                 if wg:
                     wg.conv_in(r, g)
                 dx_in = self._buf(('bwd', 'dx_in'), (self.B, self.H, self.W, self.CPAD_IN), torch.float32)
-                U.conv3x3_f16(g, self.conv_in['wT'], self.cin_total, out=dx_in)
+                U.conv3x3_f16(g, self.conv_in['wT'], self.cin_total, out=dx_in, narrow=nw)
         assert not grads, 'dangling gradients in the UNet tape'
         return dx_in
 

@@ -1,6 +1,11 @@
 """Thin Python wrappers over the UNet building-block kernels (C ABI section 4, include/ssdnerf_b200.h).
 
 Activations are NHWC fp16 tensors; weights are packed once (`pack_conv_weight`, `pack_linear_weight`).
+
+`narrow=True` selects the narrow-channel GEMM family (`ssdnerf_gemm_args.algo = 3`, csrc/gemm_tc.cu): K extents per source that are
+multiples of 8 rather than 64 (a source's last K chunk is a short slab, only its k-steps that hold data are issued) and N tiles of
+16 / 40 / 48 / 80 / 160 / 256 columns fitted to N.  The tiled-triplane UNet (80 / 160 / 320 channels, 40 / 80-wide heads) runs on it;
+every other caller keeps the default family and its 64-multiple K contract.
 """
 import ctypes
 
@@ -28,6 +33,8 @@ class GemmArgs(ctypes.Structure):
     ]
 
 
+ALGO_NARROW = 3     # ssdnerf_gemm_args.algo of the narrow-channel family
+
 GEMM_PROF = None    # set to a uint64[8] CUDA tensor to collect the generic GEMM kernel's pipeline wait cycles (debug, ssdnerf_gemm_args.debug_cycles)
 GEMM_LOG = None     # set to a list to record (M, N, K, taps, bn, cluster, batched, fused_stats) of every launch (profiling scripts)
 
@@ -49,24 +56,27 @@ def _pad_rows(w, mult=64):
     return w
 
 
-def pack_linear_weight(w):
-    """nn.Linear / 1x1-conv weight [N, K] -> fp16 [N_pad, K] (rows padded to a multiple of 64 so any N tile is in bounds)."""
+def pack_linear_weight(w, narrow=False):
+    """nn.Linear / 1x1-conv weight [N, K] -> fp16 [N_pad, K] (rows padded to a multiple of 64 so any N tile is in bounds).
+    narrow: K a multiple of 8 (the narrow-channel GEMM family)."""
     w = w.detach().reshape(w.shape[0], -1).half()
-    assert w.shape[1] % 64 == 0, 'K must be a multiple of 64'
+    assert w.shape[1] % (8 if narrow else 64) == 0, 'K must be a multiple of 64 (narrow: of 8)'
     return _pad_rows(w).contiguous()
 
 
-def pack_conv_weight(w, cin_pad=None):
-    """Conv2d weight [Cout, Cin, 3, 3] -> fp16 [9][Cout_pad][Cin_pad] (tap = ky*3 + kx, K contiguous)."""
+def pack_conv_weight(w, cin_pad=None, narrow=False):
+    """Conv2d weight [Cout, Cin, 3, 3] -> fp16 [9][Cout_pad][Cin_pad] (tap = ky*3 + kx, K contiguous).
+    Cin_pad defaults to the next multiple of 64 (narrow: of 8)."""
     cout, cin = w.shape[0], w.shape[1]
-    cin_pad = cin_pad or ((cin + 63) // 64 * 64)
+    m = 8 if narrow else 64
+    cin_pad = cin_pad or ((cin + m - 1) // m * m)
     wp = w.detach().permute(2, 3, 0, 1).reshape(9, cout, cin).half()
     if cin_pad != cin:
         wp = torch.cat([wp, wp.new_zeros(9, cout, cin_pad - cin)], dim=-1)
     return _pad_rows(wp).contiguous()
 
 
-def linear_f16(a, w, bias=None, residual=None, out=None, out_f32=False, alpha=1.0, bn=0, n=None, cluster=0, qstats=None, stats_hw=0):
+def linear_f16(a, w, bias=None, residual=None, out=None, out_f32=False, alpha=1.0, bn=0, n=None, cluster=0, qstats=None, stats_hw=0, narrow=False):
     """out[M, N] = alpha * a[M, K] @ w[N, K]^T + bias + residual.  a fp16 [M, K] (row stride may exceed K)."""
     N.require_cuda(a, w)
     M, K = a.shape
@@ -89,28 +99,52 @@ def linear_f16(a, w, bias=None, residual=None, out=None, out_f32=False, alpha=1.
     g.so1, g.so2, g.so3 = out.stride(0), 0, 0
     if qstats is not None:
         g.qstats, g.stats_hw = qstats.data_ptr(), stats_hw
+    if narrow:
+        g.algo = ALGO_NARROW
     _launch(g)
     return out
 
 
-def _conv_boxes(H, W):
+def _conv_boxes(H, W, narrow=False):
+    if narrow:
+        return _conv_boxes_narrow(H, W)
     bw = min(W, 128)
     bh = min(H, 128 // bw)
     nb = 128 // (bw * bh)
     return bw, bh, nb
 
 
-def conv3x3_f16(x, wp, cout, bias=None, x2=None, residual=None, out=None, out_f32=False, taps=9, bn=0, cluster=0, qstats=None, algo=0):
+def _pow2_floor(v):
+    return 1 << (max(int(v), 1).bit_length() - 1)
+
+
+def _conv_boxes_narrow(H, W):
+    """128-pixel TMA boxes (bw x bh x nb images, powers of two) for any H x W: the widest power of two that divides W (no partial
+    boxes along a row), rows filling the rest.  The fused quad statistics need every 64-pixel half of a box inside one image (nb <= 2);
+    where that would not hold (4 x 12) the box is the next power of two above W and H, its tail zero-filled and masked."""
+    bw = min(128, W & -W)
+    bh = min(128 // bw, _pow2_floor(H))
+    if 128 // (bw * bh) > 2:
+        bw = min(128, 1 << (W - 1).bit_length())
+        bh = min(128 // bw, 1 << (H - 1).bit_length())
+    return bw, bh, 128 // (bw * bh)
+
+
+def conv3x3_f16(x, wp, cout, bias=None, x2=None, residual=None, out=None, out_f32=False, taps=9, bn=0, cluster=0, qstats=None, algo=0,
+                narrow=False):
     """3x3 (taps=9, pad 1, stride 1) or 1x1 (taps=1) convolution over NHWC fp16 x [B,H,W,C1] (+ x2 [B,H,W,C2] concatenated
-    along channels).  wp: packed weight [taps][Cout_pad][C1+C2]."""
+    along channels).  wp: packed weight [taps][Cout_pad][C1+C2].  narrow: C1 / C2 multiples of 8 (narrow-channel family)."""
     N.require_cuda(x, wp)
     B, H, W, C1 = x.shape
     C2 = x2.shape[-1] if x2 is not None else 0
     assert x.is_contiguous() and (x2 is None or x2.is_contiguous())
-    assert wp.shape[-1] == C1 + C2 and C1 % 64 == 0 and C2 % 64 == 0, (wp.shape, C1, C2)
+    km = 8 if narrow else 64
+    assert wp.shape[-1] == C1 + C2 and C1 % km == 0 and C2 % km == 0, (wp.shape, C1, C2)
+    if narrow:
+        algo = ALGO_NARROW
     if out is None:
         out = torch.empty(B, H, W, cout, dtype=torch.float32 if out_f32 else torch.float16, device=x.device)
-    bw, bh, nb = _conv_boxes(H, W)
+    bw, bh, nb = _conv_boxes(H, W, narrow)
     g = GemmArgs()
     g.a1, g.k1 = x.data_ptr(), C1
     g.a1_strides = (c_u64 * 3)(C1 * 2, W * C1 * 2, H * W * C1 * 2)
@@ -135,16 +169,16 @@ def conv3x3_f16(x, wp, cout, bias=None, x2=None, residual=None, out=None, out_f3
     return out
 
 
-def conv3x3_s2_f16(x, wp, cout, bias=None, out=None, qstats=None):
+def conv3x3_s2_f16(x, wp, cout, bias=None, out=None, qstats=None, narrow=False):
     """3x3 stride-2 pad-1 convolution (mmgen DenoisingDownsample) over NHWC fp16 x [B,H,W,C] -> [B,H/2,W/2,cout] WITHOUT an im2col
     buffer: the same implicit GEMM as the stride-1 convolution, its TMA boxes traversing every second input pixel (a_stride = 2)."""
     N.require_cuda(x, wp)
     B, H, W, C = x.shape
-    assert x.is_contiguous() and H % 2 == 0 and W % 2 == 0 and wp.shape[-1] == C and C % 64 == 0
+    assert x.is_contiguous() and H % 2 == 0 and W % 2 == 0 and wp.shape[-1] == C and C % (8 if narrow else 64) == 0
     Ho, Wo = H // 2, W // 2
     if out is None:
         out = torch.empty(B, Ho, Wo, cout, dtype=torch.float16, device=x.device)
-    bw, bh, nb = _conv_boxes(Ho, Wo)
+    bw, bh, nb = _conv_boxes(Ho, Wo, narrow)
     g = GemmArgs()
     g.a1, g.k1 = x.data_ptr(), C
     g.a1_strides = (c_u64 * 3)(C * 2, W * C * 2, H * W * C * 2)
@@ -153,7 +187,7 @@ def conv3x3_s2_f16(x, wp, cout, bias=None, out=None, qstats=None):
     rows = wp.shape[-2]
     g.b, g.n, g.n_rows_b, g.bx2, g.bx3 = wp.data_ptr(), cout, rows, 9, 1
     g.b_strides = (c_u64 * 3)(C * 2, rows * C * 2, 9 * rows * C * 2)
-    g.bn, g.alpha, g.algo = 0, 1.0, 1
+    g.bn, g.alpha, g.algo = 0, 1.0, ALGO_NARROW if narrow else 1
     g.bias_n = bias.data_ptr() if bias is not None else None
     g.out, g.out_f32 = out.data_ptr(), int(out.dtype == torch.float32)
     g.so1, g.so2, g.so3 = cout, Wo * cout, Ho * Wo * cout
@@ -166,7 +200,7 @@ def conv3x3_s2_f16(x, wp, cout, bias=None, out=None, qstats=None):
 _UP_ROWS = {0: ((-1, (0,)), (0, (1, 2))), 1: ((0, (0, 1)), (1, (2,)))}     # output parity -> ((source offset, merged kernel rows), ...)
 
 
-def pack_upconv_weight(w):
+def pack_upconv_weight(w, narrow=False):
     """nearest-x2 upsample followed by conv3x3 == four 2x2-tap convolutions of the LOW-resolution image, one per output parity
     (py, px): kernel rows / columns that read the same source pixel are summed.  w [Cout, Cin, 3, 3] -> fp16 [4 phases][4 taps][Cout_pad][Cin]
     (phase = py*2 + px, tap = iy*2 + ix) -- 16 tap-GEMMs at a quarter of the pixels = 4/9 of the flops, and no upsampled tensor."""
@@ -180,18 +214,18 @@ def pack_upconv_weight(w):
                     taps.append(sum(w[:, :, ky, kx] for ky in kys for kx in kxs))
             phases.append(torch.stack(taps))                     # [4, Cout, Cin]
     wp = torch.stack(phases).half()                              # [4, 4, Cout, Cin]
-    assert wp.shape[-1] % 64 == 0
+    assert wp.shape[-1] % (8 if narrow else 64) == 0
     return _pad_rows(wp).contiguous()
 
 
-def upconv3x3_f16(x, wps, cout, bias=None, out=None, qstats=None):
+def upconv3x3_f16(x, wps, cout, bias=None, out=None, qstats=None, narrow=False):
     """conv3x3(nearest_x2(x)) (mmgen DenoisingUpsample) from the low-resolution x [B,H,W,C] -> [B,2H,2W,cout]; wps = pack_upconv_weight."""
     N.require_cuda(x, wps)
     B, H, W, C = x.shape
     assert x.is_contiguous() and wps.shape[-1] == C
     if out is None:
         out = torch.empty(B, 2 * H, 2 * W, cout, dtype=torch.float16, device=x.device)
-    bw, bh, nb = _conv_boxes(H, W)
+    bw, bh, nb = _conv_boxes(H, W, narrow)
     rows = wps.shape[-2]
     esz = out.element_size()
     for py in (0, 1):
@@ -207,7 +241,7 @@ def upconv3x3_f16(x, wps, cout, bias=None, out=None, qstats=None):
             g.b = wps.data_ptr() + ph * 4 * rows * C * 2
             g.n, g.n_rows_b, g.bx2, g.bx3 = cout, rows, 4, 1
             g.b_strides = (c_u64 * 3)(C * 2, rows * C * 2, 4 * rows * C * 2)
-            g.bn, g.alpha, g.algo = 0, 1.0, 1
+            g.bn, g.alpha, g.algo = 0, 1.0, ALGO_NARROW if narrow else 1
             g.bias_n = bias.data_ptr() if bias is not None else None
             g.out = out.data_ptr() + (py * 2 * W + px) * cout * esz
             g.out_f32 = int(out.dtype == torch.float32)
@@ -218,13 +252,14 @@ def upconv3x3_f16(x, wps, cout, bias=None, out=None, qstats=None):
     return out
 
 
-def attn_scores(qkv, heads, scale, out=None):
+def attn_scores(qkv, heads, scale, out=None, narrow=False):
     """S[b,h,t,s] = scale * q[b,t,h,:] . k[b,s,h,:] in fp32, q/k read in place from qkv [B,T,3c] with the reference's
-    legacy head layout (head h owns channels [h*3ch, (h+1)*3ch) = q | k | v; lib/models/architecture/ddpm/modules.py:36-48)."""
+    legacy head layout (head h owns channels [h*3ch, (h+1)*3ch) = q | k | v; lib/models/architecture/ddpm/modules.py:36-48).
+    narrow: head widths that are multiples of 8 (40, 80), K = ch zero-filled to the next 16 by TMA."""
     B, T, c3 = qkv.shape
     c = c3 // 3
     ch = c // heads
-    assert ch % 64 == 0
+    assert ch % (8 if narrow else 64) == 0
     if out is None:
         out = torch.empty(B, heads, T, T, dtype=torch.float32, device=qkv.device)
     g = GemmArgs()
@@ -238,16 +273,18 @@ def attn_scores(qkv, heads, scale, out=None):
     g.bn, g.alpha = 0, scale
     g.out, g.out_f32 = out.data_ptr(), 1
     g.so1, g.so2, g.so3 = T, T * T, heads * T * T
+    if narrow:
+        g.algo = ALGO_NARROW
     _launch(g)
     return out
 
 
-def attn_pv(P, vt, out=None):
+def attn_pv(P, vt, out=None, narrow=False):
     """O[b,t,h*ch + c] = sum_s P[b,h,t,s] * vt[b,h,c,s]   (P fp16 [B,heads,T,T], vt fp16 [B,heads,ch,T]) -> fp16 [B,T,heads*ch]"""
     B, heads, T, _ = P.shape
     ch = vt.shape[2]
     c = heads * ch
-    assert T % 64 == 0
+    assert T % (8 if narrow else 64) == 0
     if out is None:
         out = torch.empty(B, T, c, dtype=torch.float16, device=P.device)
     g = GemmArgs()
@@ -260,6 +297,8 @@ def attn_pv(P, vt, out=None):
     g.bn, g.alpha = 0, 1.0
     g.out, g.out_f32 = out.data_ptr(), 0
     g.so1, g.so2, g.so3 = c, ch, T * c
+    if narrow:
+        g.algo = ALGO_NARROW
     _launch(g)
     return out
 
@@ -323,16 +362,16 @@ def conv3x3_gn_f16(x1, q1, gamma, beta, wp, bias=None, x2=None, q2=None, scale_s
 # ---------------------------------------------------------------------------------------------------------------------
 # input-gradient pass (C ABI section 4b): data gradients of the frozen UNet
 # ---------------------------------------------------------------------------------------------------------------------
-def pack_conv_weight_dgrad(w, cout_pad=None):
+def pack_conv_weight_dgrad(w, cout_pad=None, narrow=False):
     """Conv2d weight [Cout, Cin, 3, 3] -> packed weight of the DATA-GRADIENT convolution: dX = conv3x3(dY, W^T with flipped taps),
     i.e. a 3x3 stride-1 convolution whose input channels are Cout (zero-padded to `cout_pad`) and whose outputs are Cin."""
-    return pack_conv_weight(w.detach().transpose(0, 1).flip(2, 3), cin_pad=cout_pad)
+    return pack_conv_weight(w.detach().transpose(0, 1).flip(2, 3), cin_pad=cout_pad, narrow=narrow)
 
 
-def pack_linear_weight_dgrad(w):
+def pack_linear_weight_dgrad(w, narrow=False):
     """Linear / 1x1-conv weight [N, K] -> packed [K_pad, N] so that dX[M, K] = dY[M, N] @ W."""
     w = w.detach().reshape(w.shape[0], -1)
-    return pack_linear_weight(w.t())
+    return pack_linear_weight(w.t(), narrow=narrow)
 
 
 class GnBwdArgs(ctypes.Structure):
@@ -347,8 +386,8 @@ class GnBwdArgs(ctypes.Structure):
 
 
 def gn_bwd(x1, x2, stats, gamma, beta, dy, dx1, dx2=None, add=None, scale_shift_ptr=None, ss_batch_stride=0, silu=True, gsum=None, eps=1e-5,
-           csum=None):
-    """GroupNorm(32)(+scale/shift)(+SiLU) backward over the channel concat of x1 (+x2); stats = (quad_flag, s1, s2) as the forward used.
+           csum=None, groups=32):
+    """GroupNorm(groups)(+scale/shift)(+SiLU) backward over the channel concat of x1 (+x2); stats = (quad_flag, s1, s2) as the forward used.
     csum (fp32 [B, C, 2], overwritten): per-(image, channel) sums the affine / scale-shift parameter gradients are built from."""
     N.require_cuda(x1, dy, dx1)
     B, H, W, C1 = x1.shape
@@ -356,7 +395,7 @@ def gn_bwd(x1, x2, stats, gamma, beta, dy, dx1, dx2=None, add=None, scale_shift_
     a.x1, a.C1 = x1.data_ptr(), C1
     if x2 is not None:
         a.x2, a.C2 = x2.data_ptr(), x2.shape[-1]
-    a.B, a.HW, a.groups = B, H * W, 32
+    a.B, a.HW, a.groups = B, H * W, groups
     quad, s1, s2 = stats
     a.stats, a.quad_stats = s1.data_ptr(), int(quad)
     a.stats2 = s2.data_ptr() if s2 is not None else None
@@ -367,7 +406,7 @@ def gn_bwd(x1, x2, stats, gamma, beta, dy, dx1, dx2=None, add=None, scale_shift_
     a.dy = dy.data_ptr()
     a.add = add.data_ptr() if add is not None else None
     if gsum is None:
-        gsum = torch.empty(B * 32 * 2, dtype=torch.float32, device=x1.device)
+        gsum = torch.empty(B * groups * 2, dtype=torch.float32, device=x1.device)
     a.group_sums = gsum.data_ptr()
     a.dx1 = dx1.data_ptr()
     a.dx2 = dx2.data_ptr() if dx2 is not None else None
@@ -419,7 +458,7 @@ def transpose_f16(src_ptr, dst, rows, cols, row_stride, stride1, n1, stride2, n2
     return dst
 
 
-def _bgemm(a_ptr, a_strides, k, b_ptr, b_strides, n, T, heads, B, out_ptr, out_strides, out_f32, alpha):
+def _bgemm(a_ptr, a_strides, k, b_ptr, b_strides, n, T, heads, B, out_ptr, out_strides, out_f32, alpha, narrow=False):
     """batched GEMM over (head, batch): out[b,h,t,:n] = alpha * A[b,h,t,:k] @ Bm[b,h,:n,:k]^T (strides in bytes for A / Bm, elements for out)"""
     g = GemmArgs()
     g.a1, g.k1 = a_ptr, k
@@ -431,24 +470,26 @@ def _bgemm(a_ptr, a_strides, k, b_ptr, b_strides, n, T, heads, B, out_ptr, out_s
     g.bn, g.alpha = 0, alpha
     g.out, g.out_f32 = out_ptr, int(out_f32)
     g.so1, g.so2, g.so3 = out_strides
+    if narrow:
+        g.algo = ALGO_NARROW
     _launch(g)
 
 
-def attn_backward(qkv, d_o, heads, scale, ws):
+def attn_backward(qkv, d_o, heads, scale, ws, narrow=False):
     """Attention data gradient (softmax(scale q k^T) v, legacy head layout of modules.py:36-48) by recomputation on the tensor cores:
     qkv fp16 [B,T,3c] (saved by the forward), d_o fp16 [B,T,c] -> dqkv fp16 [B,T,3c].  `ws(name, shape, dtype)` supplies scratch."""
     B, T, c3 = qkv.shape
     c = c3 // 3
     ch = c // heads
     L, s = N.lib(), N.stream_ptr
-    S = attn_scores(qkv, heads, scale, out=ws('S', (B, heads, T, T), torch.float32))
+    S = attn_scores(qkv, heads, scale, out=ws('S', (B, heads, T, T), torch.float32), narrow=narrow)
     P = ws('P', (B, heads, T, T), torch.float16)
     N.check(L.ssdnerf_softmax_rows(N.ptr(S), N.c_u32(B * heads * T), N.c_u32(T), N.ptr(P), s()))
     qp, dop = qkv.data_ptr(), d_o.data_ptr()
     TT = T * T
     # dP[b,h,t,s] = d_o[b,t,h,:] . v[b,s,h,:]   (into the score buffer, which is dead after the softmax)
     _bgemm(dop, (c * 2, ch * 2, T * c * 2), ch, qp + 2 * ch * 2, (c3 * 2, 3 * ch * 2, T * c3 * 2), T, T, heads, B,
-           S.data_ptr(), (T, TT, heads * TT), True, 1.0)
+           S.data_ptr(), (T, TT, heads * TT), True, 1.0, narrow)
     dS = ws('dS', (B, heads, T, T), torch.float16)
     N.check(L.ssdnerf_softmax_bwd_rows(N.ptr(P), N.ptr(S), N.c_u32(B * heads * T), N.c_u32(T), N.ptr(dS), s()))
     Pt = transpose_f16(P.data_ptr(), ws('Pt', (B, heads, T, T), torch.float16), T, T, T, TT, heads, heads * TT, B)
@@ -461,9 +502,9 @@ def attn_backward(qkv, d_o, heads, scale, ws):
     b_ct = (T * 2, ch * T * 2, heads * ch * T * 2)
     o_str = (c3, 3 * ch, T * c3)
     dp = dqkv.data_ptr()
-    _bgemm(dS.data_ptr(), a_tt, T, kt.data_ptr(), b_ct, ch, T, heads, B, dp, o_str, False, scale)                  # dq = scale dS k
-    _bgemm(dSt.data_ptr(), a_tt, T, qt.data_ptr(), b_ct, ch, T, heads, B, dp + ch * 2, o_str, False, scale)        # dk = scale dS^T q
-    _bgemm(Pt.data_ptr(), a_tt, T, dot.data_ptr(), b_ct, ch, T, heads, B, dp + 2 * ch * 2, o_str, False, 1.0)      # dv = P^T d_o
+    _bgemm(dS.data_ptr(), a_tt, T, kt.data_ptr(), b_ct, ch, T, heads, B, dp, o_str, False, scale, narrow)          # dq = scale dS k
+    _bgemm(dSt.data_ptr(), a_tt, T, qt.data_ptr(), b_ct, ch, T, heads, B, dp + ch * 2, o_str, False, scale, narrow)  # dk = scale dS^T q
+    _bgemm(Pt.data_ptr(), a_tt, T, dot.data_ptr(), b_ct, ch, T, heads, B, dp + 2 * ch * 2, o_str, False, 1.0, narrow)  # dv = P^T d_o
     return dqkv
 
 

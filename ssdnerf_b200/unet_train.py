@@ -30,10 +30,23 @@ def _pad64(c):
     return (c + 63) // 64 * 64
 
 
+def check_trainable(m):
+    """the weight-gradient pass covers what every paper config uses: widths that are multiples of 64 and GroupNorm(32).  Anything else
+    (the tiled-triplane config's 80 / 160 / 320 channels with GroupNorm(16)) raises naming itself; its sampling, guidance and
+    guide_optim run natively."""
+    from .unet import is_narrow, unet_widths
+    if is_narrow(m) or m.num_groups != 32:
+        raise NotImplementedError(f'training the denoiser with channel widths {unet_widths(m)} and GroupNorm({m.num_groups}) is not built: the '
+                                  f'weight-gradient pass covers widths that are multiples of 64 with GroupNorm(32), not the tiled-triplane '
+                                  f'config\'s 80 / 160 / 320 channels with GroupNorm(16); sampling, guidance and guide_optim run natively')
+
+
 class WeightGradPass:
-    """Collects parameter gradients during one walk of the tape.  `grads[param] = fp32 tensor in the parameter's shape`."""
+    """Collects parameter gradients during one walk of the tape.  `grads[param] = fp32 tensor in the parameter's shape`.
+    Models outside `check_trainable` are refused."""
 
     def __init__(self, eng):
+        check_trainable(eng.m)
         self.eng = eng
         self.grads = {}
         self.d_ss = torch.zeros(eng.B, eng.ss_total, dtype=torch.float32, device=eng.dev)
@@ -97,11 +110,11 @@ class WeightGradPass:
         ss = N.c_void_p(eng.ss_cur.data_ptr() + 4 * ss_off) if ss_off is not None else None
         quad, s1, s2 = st
         if quad:
-            N.check(L.ssdnerf_gn_apply_q(N.ptr(x1), N.c_u32(C1), N.ptr(x2), N.c_u32(C2), N.c_u32(B), N.c_u32(H * W), N.c_u32(32), N.ptr(s1),
+            N.check(L.ssdnerf_gn_apply_q(N.ptr(x1), N.c_u32(C1), N.ptr(x2), N.c_u32(C2), N.c_u32(B), N.c_u32(H * W), N.c_u32(eng.groups), N.ptr(s1),
                                          N.ptr(s2), N.ptr(gamma), N.ptr(beta), ss, N.c_longlong(eng.ss_total), N.c_f32(1e-5),
                                          N.c_int(int(silu)), N.ptr(out), s))
         else:
-            N.check(L.ssdnerf_gn_apply(N.ptr(x1), N.c_u32(C1), N.ptr(x2), N.c_u32(C2), N.c_u32(B), N.c_u32(H * W), N.c_u32(32), N.ptr(s1),
+            N.check(L.ssdnerf_gn_apply(N.ptr(x1), N.c_u32(C1), N.ptr(x2), N.c_u32(C2), N.c_u32(B), N.c_u32(H * W), N.c_u32(eng.groups), N.ptr(s1),
                                        N.ptr(gamma), N.ptr(beta), ss, N.c_longlong(eng.ss_total), N.c_f32(1e-5), N.c_int(int(silu)),
                                        N.ptr(out), s))
         return out
@@ -180,7 +193,7 @@ class _UNetFullGrad(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x_t, module, t, *params):
         B = x_t.shape[0]
-        eng = module.engine(B, x_t.device)
+        eng = module.engine(B, x_t.device, x_t.shape[-2:])
         with torch.enable_grad():       # tiny differentiable graph: time embedding -> per-block (scale, shift) rows
             emb = module.embedding(t.to(x_t.device))
             ss = eng.scale_shift_rows(emb, live=True)
@@ -208,6 +221,7 @@ class _UNetFullGrad(torch.autograd.Function):
 
 
 def forward_with_weight_grads(module, x_t, t):
+    check_trainable(module)       # refuse before the forward rather than in the backward
     if module.concat_cond_channels > 0:
         raise NotImplementedError('training with concat_cond (image_cond) is not built (unused by the shipped configs)')
     return _UNetFullGrad.apply(x_t, module, t, *module.parameters())
