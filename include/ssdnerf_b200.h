@@ -248,7 +248,6 @@ typedef struct ssdnerf_gemm_args {
      *    conv / plain: coordinate 2 = tap; b_batched: coordinates (2, 3) = the tile's (d2, d3) tile indices */
     const void* b; uint64_t b_strides[3]; uint32_t n, n_rows_b, bx2, bx3; uint32_t b_batched;
     uint32_t bn;              /* N tile: 0 = auto, else 64 / 128 / 256 */
-    uint32_t cluster;         /* 0 = auto (no cluster), 1 = no cluster, 2 / 4 / 8 = clusters along M with TMA multicast of the B tile */
     float alpha;
     const float* bias_n;      /* [n] fp32 or NULL */
     const void* residual;     /* fp16, addressed like out, or NULL */
@@ -256,12 +255,9 @@ typedef struct ssdnerf_gemm_args {
     /* optional fused GroupNorm statistics of the output: qstats [images][n/4][2] += {sum, sum of squares} of every 4-channel quad
      * (caller zero-fills); image of a row = index along d3 (stats_hw == 0) or (index along d1) / stats_hw (flattened rows) */
     float* qstats; uint32_t stats_hw;
-    void* debug_cycles;      /* optional uint64[8] device counters of the generic tile kernel, clock cycles summed over CTAs: [0] producer wait
-                              * for a free stage, [1] producer total, [2] consumer wait for a full stage, [4] consumer total; NULL in production */
     uint32_t algo;           /* 0 = auto, 1 = generic tile kernel, 2 = row-pair 3x3 convolution (128-pixel rows, 128 output channels),
                               * 3 = narrow-channel family: k1 / k2 multiples of 8 (a source's last K chunk is a short slab, only its
-                              * k-steps that hold data are issued), N tiles of 16 / 40 / 48 / 80 / 160 / 256 fitted to n (bn 0 = auto),
-                              * no clusters */
+                              * k-steps that hold data are issued), N tiles of 16 / 40 / 48 / 80 / 160 / 256 fitted to n (bn 0 = auto) */
     /* generalised K-slabs: taps in [1, 9] with tap_offsets[2t], [2t+1] = shift of slab t in (d1, d2) (NULL: the 3x3 / 1x1 defaults) --
      * e.g. the four 2x2-tap phase convolutions a nearest-x2 upsample + 3x3 convolution decomposes into;
      * a_stride 2 = stride-2 convolution: (d1, d2) are output extents, a1 / a2 describe the (2 d1 x 2 d2) input read at every 2nd pixel */
@@ -286,31 +282,6 @@ SSDNERF_API int ssdnerf_gn_apply_q(const void* x1, uint32_t C1, const void* x2, 
 SSDNERF_API int ssdnerf_gn_apply(const void* x1, uint32_t C1, const void* x2, uint32_t C2, uint32_t B, uint32_t HW, uint32_t groups,
                                  const float* stats, const float* gamma, const float* beta, const float* scale_shift,
                                  long long ss_batch_stride, float eps, int do_silu, void* out, void* stream);
-/* [B,H,W,C] -> [B,H/2,W/2,9C] patches of a 3x3 stride-2 pad-1 convolution (DenoisingDownsample), K index = tap*C + c */
-SSDNERF_API int ssdnerf_im2col_s2(const void* x, uint32_t B, uint32_t H, uint32_t W, uint32_t C, void* out, void* stream);
-/* nearest-neighbour x2 (DenoisingUpsample) */
-SSDNERF_API int ssdnerf_upsample2x(const void* x, uint32_t B, uint32_t H, uint32_t W, uint32_t C, void* out, void* stream);
-/* Fused GroupNorm(32) (+ NormWithEmbedding scale/shift) + SiLU + 3x3 convolution, 128-pixel-wide images, 128 output channels
- * (the UNet's 128 x 128 level).  replaces: mmgen DenoisingResBlock's `conv(act(norm(x)))` pairs as used by
- * lib/models/architecture/ddpm/modules.py:51-110 -- GroupNorm apply + SiLU + Conv2d, without materialising the normalised activation.
- * x1 (+ x2, channel concat) are the RAW NHWC fp16 tensors; q1 / q2 their quad statistics as emitted by ssdnerf_gemm_f16 (qstats). */
-typedef struct ssdnerf_conv_gn_args {
-    const void* x1; uint32_t C1;          /* [B][H][128][C1] fp16 */
-    const void* x2; uint32_t C2;          /* optional second input [B][H][128][C2] */
-    uint32_t B, H;                         /* H even */
-    const float* q1; const float* q2;      /* [B][C/4][2] */
-    const float* gamma; const float* beta; /* [C1 + C2] */
-    const float* scale_shift;              /* optional [B][...]: row b holds scale[C] | shift[C] at scale_shift + b * ss_batch_stride */
-    long long ss_batch_stride;
-    float eps;
-    const void* w; uint32_t w_rows;        /* packed fp16 weight [9][w_rows >= 128][C1 + C2] */
-    const float* bias;                     /* [128] or NULL */
-    const void* residual;                  /* [B][H][128][128] fp16 or NULL */
-    void* out;                             /* [B][H][128][128] fp16 */
-    float* qstats;                         /* optional [B][32][2] quad statistics of the output (caller zero-fills) */
-    void* coef_workspace;                  /* device scratch, B * (C1 + C2) * 8 bytes, 16-byte aligned (per-image affine table) */
-} ssdnerf_conv_gn_args;
-SSDNERF_API int ssdnerf_conv3x3_gn_f16(const ssdnerf_conv_gn_args* args, void* stream);
 /* fused attention: out[b][t][h*ch + d] = softmax_s(scale * q[b,t,h,:] . k[b,s,h,:]) v[b,s,h,d], scores kept on chip (flash-style);
  * qkv fp16 [B][T][3*heads*ch] with the legacy head layout (modules.py:36-48), ch in {64, 128}, T % 64 == 0 */
 SSDNERF_API int ssdnerf_flash_attn(const void* qkv, uint32_t B, uint32_t T, uint32_t heads, uint32_t ch, float scale, void* out, void* stream);
@@ -357,9 +328,12 @@ SSDNERF_API int ssdnerf_softmax_bwd_rows(const void* P, const float* dP, uint32_
 /* n2 x n1 batched fp16 transposes: dst[((b2*n1 + b1)*cols + c)*rows + r] = src[b2*stride2 + b1*stride1 + r*row_stride + c] (elements) */
 SSDNERF_API int ssdnerf_transpose_f16(const void* src, void* dst, uint32_t rows, uint32_t cols, long long row_stride, long long stride1,
                                       uint32_t n1, long long stride2, uint32_t n2, void* stream);
-/* data gradient of ssdnerf_im2col_s2 (+ optional add [B][H][W][C]): dcol fp16 [B][H/2][W/2][9C] -> dx fp16 [B][H][W][C] */
+/* data gradient of the 3x3 stride-2 pad-1 patch gather (K index = tap*C + c): dx[b][y][x][c] = sum of dcol[b][oy][ox][tap*C + c] over the
+ * (oy, ox, tap) with 2 oy + tap/3 - 1 == y and 2 ox + tap%3 - 1 == x (+ optional add [B][H][W][C]);
+ * dcol fp16 [B][H/2][W/2][9C] -> dx fp16 [B][H][W][C] */
 SSDNERF_API int ssdnerf_col2im_s2(const void* dcol, uint32_t B, uint32_t H, uint32_t W, uint32_t C, const void* add, void* dx, void* stream);
-/* data gradient of ssdnerf_upsample2x: dup fp16 [B][2H][2W][C] -> dx fp16 [B][H][W][C] */
+/* data gradient of a nearest-neighbour x2 upsample: dx[b][y][x][c] = sum of the 2x2 block dup[b][2y..2y+1][2x..2x+1][c];
+ * dup fp16 [B][2H][2W][C] -> dx fp16 [B][H][W][C] */
 SSDNERF_API int ssdnerf_sum2x2(const void* dup, uint32_t B, uint32_t H, uint32_t W, uint32_t C, void* dx, void* stream);
 /* dst += src over n fp16 elements (n % 8 == 0) */
 SSDNERF_API int ssdnerf_add_f16(void* dst, const void* src, unsigned long long n, void* stream);

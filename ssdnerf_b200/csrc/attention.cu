@@ -11,11 +11,11 @@
 #include "common.cuh"
 #include "../../include/ssdnerf_b200.h"
 #include <cuda_fp16.h>
-#include <cstdlib>
 
 namespace ssdnerf {
 
-constexpr int kFaBN = 64;      // keys per shared-memory tile; queries per CTA = 16 per warp, WARPS in {4, 8}
+constexpr int kFaBN = 64;      // keys per shared-memory tile
+constexpr int kFaWarps = 4;    // queries per CTA = 16 per warp
 
 __device__ __forceinline__ void fa_cp_async16(uint32_t dst, const void* src) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" :: "r"(dst), "l"(src) : "memory");
@@ -35,18 +35,18 @@ __device__ __forceinline__ void fa_mma(float* d, const uint32_t* a, uint32_t b0,
 __device__ __forceinline__ uint32_t fa_pack(float a, float b) { const __half2 h = __floats2half2_rn(a, b); return *reinterpret_cast<const uint32_t*>(&h); }
 __device__ __forceinline__ float fa_exp2(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 
-// grid (T / (16 WARPS), B * heads); qkv fp16 [B][T][3 * heads * CH]; out fp16 [B][T][heads * CH]
-template <int CH, int WARPS>
-__global__ void __launch_bounds__(WARPS * 32) k_flash_attn(const __half* __restrict__ qkv, uint32_t T, uint32_t heads, float scale_log2,
+// grid (T / (16 kFaWarps), B * heads); qkv fp16 [B][T][3 * heads * CH]; out fp16 [B][T][heads * CH]
+template <int CH>
+__global__ void __launch_bounds__(kFaWarps * 32) k_flash_attn(const __half* __restrict__ qkv, uint32_t T, uint32_t heads, float scale_log2,
                                                            __half* __restrict__ out) {
-    constexpr int kFaThreads = WARPS * 32, kFaBM = WARPS * 16;
+    constexpr int kFaThreads = kFaWarps * 32, kFaBM = kFaWarps * 16;
     constexpr int kRow = CH * 2 + 16;                 // bytes per smem row (16 B pad: conflict-free ldmatrix)
     constexpr int kTile = kFaBN * kRow;               // one 64-row K / V tile
     constexpr int kQBytes = kFaBM * kRow;
     constexpr int kKC = CH / 16;                      // k-chunks of the QK^T product
     constexpr int kVec = CH / 8;                      // 16-byte vectors per row
     extern __shared__ __align__(16) unsigned char fa_smem[];
-    unsigned char* sQ = fa_smem;                      // [16 WARPS][kRow]
+    unsigned char* sQ = fa_smem;                      // [16 kFaWarps][kRow]
     unsigned char* sK = fa_smem + kQBytes;            // [2][64][kRow]
     unsigned char* sV = sK + 2 * kTile;               // [2][64][kRow]
 
@@ -157,14 +157,14 @@ __global__ void __launch_bounds__(WARPS * 32) k_flash_attn(const __half* __restr
     }
 }
 
-template <int CH, int WARPS>
+template <int CH>
 static int launch_flash(const __half* qkv, uint32_t B, uint32_t T, uint32_t heads, float scale, __half* out, cudaStream_t stream) {
-    constexpr size_t smem = (size_t)(WARPS * 16 + 4 * kFaBN) * (CH * 2 + 16);
+    constexpr size_t smem = (size_t)(kFaWarps * 16 + 4 * kFaBN) * (CH * 2 + 16);
     static DeviceOnce attr;
     if (attr.first()) {
-        SSDNERF_CUDA_OK(cudaFuncSetAttribute(k_flash_attn<CH, WARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        SSDNERF_CUDA_OK(cudaFuncSetAttribute(k_flash_attn<CH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
-    SSDNERF_CUDA_OK(launch_pdl(k_flash_attn<CH, WARPS>, dim3(T / (WARPS * 16), B * heads), dim3(WARPS * 32), smem, stream, qkv, T, heads,
+    SSDNERF_CUDA_OK(launch_pdl(k_flash_attn<CH>, dim3(T / (kFaWarps * 16), B * heads), dim3(kFaWarps * 32), smem, stream, qkv, T, heads,
                                scale * 1.4426950408889634f, out));
     SSDNERF_LAUNCH_OK();
     return 0;
@@ -179,13 +179,7 @@ extern "C" int ssdnerf_flash_attn(const void* qkv, uint32_t B, uint32_t T, uint3
     if (!qkv || !out) return set_error_msg(SSDNERF_ERR_ARG, "flash_attn: NULL buffer");
     if (T % 64) return set_error_msg(SSDNERF_ERR_ARG, "flash_attn: T must be a multiple of 64");
     if (((uintptr_t)qkv & 15u) || ((uintptr_t)out & 3u)) return set_error_msg(SSDNERF_ERR_ARG, "flash_attn: qkv must be 16-byte aligned");
-    // 128 queries per CTA (8 warps) when the sequence is long enough to still fill the GPU, else 64 (SSDNERF_FA_WARPS=4|8 overrides)
-    static int force = -1;
-    if (force < 0) { const char* e = getenv("SSDNERF_FA_WARPS"); force = e ? atoi(e) : 0; }
-    const bool wide = force == 8 && T % 128 == 0;      // 4 warps (64 queries per CTA) is the default
-    if (ch == 64) return wide ? launch_flash<64, 8>((const __half*)qkv, B, T, heads, scale, (__half*)out, (cudaStream_t)stream)
-                              : launch_flash<64, 4>((const __half*)qkv, B, T, heads, scale, (__half*)out, (cudaStream_t)stream);
-    if (ch == 128) return wide ? launch_flash<128, 8>((const __half*)qkv, B, T, heads, scale, (__half*)out, (cudaStream_t)stream)
-                               : launch_flash<128, 4>((const __half*)qkv, B, T, heads, scale, (__half*)out, (cudaStream_t)stream);
+    if (ch == 64) return launch_flash<64>((const __half*)qkv, B, T, heads, scale, (__half*)out, (cudaStream_t)stream);
+    if (ch == 128) return launch_flash<128>((const __half*)qkv, B, T, heads, scale, (__half*)out, (cudaStream_t)stream);
     return set_error_msg(SSDNERF_ERR_ARG, "flash_attn: head width must be 64 or 128 channels");
 }

@@ -1,16 +1,13 @@
 // 3x3 convolution for the UNet's 128 x 128 level (128-pixel rows, 128 output channels): row-pair kernel with horizontal and vertical
-// halo reuse, optionally fused with the GroupNorm(32) [+ NormWithEmbedding scale / shift] + SiLU that precedes the convolution.
+// halo reuse.
 //
-// Replaces on the reference path (mmgen DenoisingResBlock.forward as used by lib/models/architecture/ddpm/modules.py:51-110):
-//     conv3x3(x)  and  conv3x3( SiLU( GroupNorm(x) * (1 + scale) + shift ) )  -- the latter without materialising the normalised input.
+// Replaces on the reference path (mmgen DenoisingResBlock.forward as used by lib/models/architecture/ddpm/modules.py:51-110): conv3x3(x).
 //
 // A tile is TWO output rows (y0, y0 + 1) of one image.  Per 64-channel chunk, the loader warpgroup reads the 4 input rows y0-1 .. y0+2
-// (130 pixels each, x = -1 .. 128, zero outside the image) ONCE, applies the GroupNorm affine a x + b in fp32 and SiLU as h + h tanh(h),
-// h = u / 2, on packed halves (tanh.approx.f16x2) when fused, and stores them in the K-major SWIZZLE_128B row layout (16-byte chunk index
-// XOR (pixel & 7)).  Zero padding is written as literal zeros (it pads the activation, not the raw input).  Consumer warpgroup a
-// accumulates output row y0 + a (2 x 64 pixels x 128 channels, fp32 in registers): for tap (ky, kx) it reads its A fragments from input
-// row ky + a shifted by kx pixels with ldmatrix and issues register-A wgmma against the tap's 128 x 64 weight tile (TMA, SWIZZLE_128B).
-// Every staged input row serves up to 6 taps, every weight tile both output rows.
+// (130 pixels each, x = -1 .. 128, zero outside the image) ONCE and stores them in the K-major SWIZZLE_128B row layout (16-byte chunk
+// index XOR (pixel & 7)).  Consumer warpgroup a accumulates output row y0 + a (2 x 64 pixels x 128 channels, fp32 in registers): for
+// tap (ky, kx) it reads its A fragments from input row ky + a shifted by kx pixels with ldmatrix and issues register-A wgmma against
+// the tap's 128 x 64 weight tile (TMA, SWIZZLE_128B).  Every staged input row serves up to 6 taps, every weight tile both output rows.
 #include "common.cuh"
 #include "tc_common.cuh"
 #include "conv_row_epilogue.cuh"
@@ -24,7 +21,6 @@ constexpr int kRwThreads = 384;                          // warpgroups 0, 1: con
 constexpr int kRwRowSlot = 17 * 1024;                    // one staged input row: 130 pixels x 64 halves = 16.25 KB, 1024-aligned slots
 constexpr int kRwBSlot = kRwN * 128;                     // 16 KB weight tile (128 output channels x 64 input channels)
 constexpr int kRwRows = 6, kRwBStages = 6;
-constexpr int kGnMaxC = 384;
 constexpr size_t kRwSmem = (size_t)kRwRows * kRwRowSlot + (size_t)kRwBStages * kRwBSlot + 1024 /*align*/ + 256 /*barriers*/ +
                            256 /*qacc*/ + 512 /*bias*/;
 
@@ -33,14 +29,12 @@ struct ConvRowParams {
     const __half* x1; uint32_t C1;              // input [B][H][128][C1] addressed with element strides xs1 {pixel, row, image}
     const __half* x2; uint32_t C2;              // optional second input (skip concat along channels)
     long long xs1[3], xs2[3];
-    const float2* coef;                         // fused GroupNorm: [B][C1 + C2] per-(image, channel) affine {a, b} from k_gn_coef; NULL: plain
     const float* bias;                          // [128] or NULL
     const __half* residual;                     // NHWC [B][H][128][128] or NULL
     __half* out;                                // NHWC [B][H][128][128]
     float* qstats;                              // optional [B][32][2]
 };
 
-template <bool GN>
 __global__ void __launch_bounds__(kRwThreads, 1)
 k_conv_row2(const __grid_constant__ CUtensorMap mapB, const ConvRowParams p) {
     extern __shared__ uint8_t smem_raw[];
@@ -74,11 +68,10 @@ k_conv_row2(const __grid_constant__ CUtensorMap mapB, const ConvRowParams p) {
     pdl_wait();
 
     // register budget: setmaxnreg moves registers within the CTA's launch-time pool (384 x 168): 128 x 120 + 256 x 192 = 384 x 168 (no spills in either role)
-    if (wg == 2) {   // ---------------- row loaders: raw rows -> (GroupNorm affine + SiLU) -> swizzled operand rows
+    if (wg == 2) {   // ---------------- row loaders: raw rows -> swizzled operand rows
         setmaxnreg_dec<120>();
         const uint32_t lt = threadIdx.x - 256u;                       // 0..127
         const uint32_t c8 = lt & 7u, p0 = lt >> 3;                    // 16-byte chunk (8 channels) of the 64-channel row; pixels p0 + 16 n
-        const uint32_t C = p.C1 + p.C2;
         uint32_t idx = 0;                                             // ring position of the row being produced
         for (uint32_t tile = tile0; tile < total_tiles; tile += tstep) {
             const uint32_t b = tile / tiles_per_img, y0 = (tile - b * tiles_per_img) * 2;
@@ -87,15 +80,6 @@ k_conv_row2(const __grid_constant__ CUtensorMap mapB, const ConvRowParams p) {
                 const __half* src = first ? p.x1 : p.x2;
                 const long long xs0 = first ? p.xs1[0] : p.xs2[0], xs1 = first ? p.xs1[1] : p.xs2[1], xs2 = first ? p.xs1[2] : p.xs2[2];
                 const uint32_t cl = (first ? j : j - kc1) * 64u + c8 * 8u;
-                float ca[8], cb[8];
-                if (GN) {   // {a, b} of this thread's 8 channels, halved: SiLU(u) = h + h tanh(h) with h = u / 2
-                    const float4* cp = reinterpret_cast<const float4*>(p.coef + (size_t)b * C + j * 64u + c8 * 8u);
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        const float4 t = __ldg(cp + k);
-                        ca[2 * k] = 0.5f * t.x; cb[2 * k] = 0.5f * t.y; ca[2 * k + 1] = 0.5f * t.z; cb[2 * k + 1] = 0.5f * t.w;
-                    }
-                }
                 for (uint32_t r = 0; r < 4; ++r) {
                     const int y = (int)(y0 + r) - 1;
                     const bool row_ok = y >= 0 && y < (int)p.H;
@@ -114,22 +98,7 @@ k_conv_row2(const __grid_constant__ CUtensorMap mapB, const ConvRowParams p) {
                     for (int n = 0; n < 9; ++n) {
                         const uint32_t px = p0 + 16u * n;
                         if (px >= 130u) continue;
-                        uint4 o = v[n];
-                        if (GN) {
-                            const bool ok = row_ok && (unsigned)((int)px - 1) < (unsigned)kRwW;
-                            const __half2* h = reinterpret_cast<const __half2*>(&v[n]);
-                            uint32_t* ow = reinterpret_cast<uint32_t*>(&o);
-#pragma unroll
-                            for (int k = 0; k < 4; ++k) {
-                                const float2 tt = __half22float2(h[k]);
-                                const __half2 hh = __floats2half2_rn(fmaf(tt.x, ca[2 * k], cb[2 * k]), fmaf(tt.y, ca[2 * k + 1], cb[2 * k + 1]));
-                                uint32_t hv = *reinterpret_cast<const uint32_t*>(&hh), tv;
-                                asm("tanh.approx.f16x2 %0, %1;" : "=r"(tv) : "r"(hv));
-                                const __half2 yy = __hfma2(hh, *reinterpret_cast<const __half2*>(&tv), hh);
-                                ow[k] = ok ? *reinterpret_cast<const uint32_t*>(&yy) : 0u;
-                            }
-                        }
-                        sts128(dst + px * 128u + ((c8 ^ (px & 7u)) << 4), o);
+                        sts128(dst + px * 128u + ((c8 ^ (px & 7u)) << 4), v[n]);
                     }
                     __syncwarp();
                     if (lane == 0) mbar_arrive(&fullR[slot]);
@@ -236,50 +205,17 @@ k_conv_row2(const __grid_constant__ CUtensorMap mapB, const ConvRowParams p) {
     __syncthreads();
 }
 
-// per-(image, channel) GroupNorm affine, k_gn_apply arithmetic: y = x * a + b,
-//   a = rstd * gamma * (1 + scale), b = (beta - mean * rstd * gamma) * (1 + scale) + shift;  grid = images, one thread per channel (looped)
-__global__ void k_gn_coef(const float* __restrict__ q1, uint32_t C1, const float* __restrict__ q2, uint32_t C2, uint32_t HW,
-                          const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ scale_shift,
-                          long long ss_batch_stride, float eps, float2* __restrict__ coef) {
-    pdl_trigger();
-    pdl_wait();
-    __shared__ float2 s_mr[32];
-    const uint32_t b = blockIdx.x, C = C1 + C2, cpg = C / 32u;
-    const float inv_n = 1.0f / ((float)HW * (float)cpg);
-    if (threadIdx.x < 32u) {
-        const uint32_t q1n = C1 / 4, q2n = C2 / 4, nq = cpg / 4;
-        float sm = 0.0f, sq = 0.0f;
-        for (uint32_t i = 0; i < nq; ++i) {
-            const uint32_t qi = threadIdx.x * nq + i;
-            const float2 t = __ldg(reinterpret_cast<const float2*>(qi < q1n ? q1 + ((size_t)b * q1n + qi) * 2 : q2 + ((size_t)b * q2n + (qi - q1n)) * 2));
-            sm += t.x; sq += t.y;
-        }
-        const float mean = sm * inv_n;
-        s_mr[threadIdx.x] = make_float2(mean, rsqrtf(fmaxf(sq * inv_n - mean * mean, 0.0f) + eps));
-    }
-    __syncthreads();
-    const float* ss = scale_shift ? scale_shift + (size_t)b * ss_batch_stride : nullptr;
-    for (uint32_t c = threadIdx.x; c < C; c += blockDim.x) {
-        const float2 mr = s_mr[c / cpg];
-        const float ak = mr.y * __ldg(gamma + c);
-        const float bk = __ldg(beta + c) - mr.x * ak;
-        const float sc = ss ? 1.0f + __ldg(ss + c) : 1.0f, sh = ss ? __ldg(ss + C + c) : 0.0f;
-        coef[(size_t)b * C + c] = make_float2(ak * sc, fmaf(bk, sc, sh));
-    }
-}
-
 // tensor-map helper shared with gemm_tc.cu
 int make_map_4d_box(CUtensorMap* m, const void* base, uint64_t K, uint64_t e1, uint64_t e2, uint64_t e3, uint64_t s1, uint64_t s2, uint64_t s3,
                     uint32_t x1, uint32_t x2, uint32_t x3);
 
-template <bool GN>
 static int launch_row2(const CUtensorMap& mB, const ConvRowParams& p, int sms, cudaStream_t stream) {
     static DeviceOnce attr;
     if (attr.first()) {
-        SSDNERF_CUDA_OK(cudaFuncSetAttribute(k_conv_row2<GN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRwSmem));
+        SSDNERF_CUDA_OK(cudaFuncSetAttribute(k_conv_row2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRwSmem));
     }
     const uint32_t total = p.B * (p.H / 2);
-    SSDNERF_CUDA_OK(launch_pdl(k_conv_row2<GN>, dim3(total < (uint32_t)sms ? total : (uint32_t)sms), dim3(kRwThreads), kRwSmem, stream, mB, p));
+    SSDNERF_CUDA_OK(launch_pdl(k_conv_row2, dim3(total < (uint32_t)sms ? total : (uint32_t)sms), dim3(kRwThreads), kRwSmem, stream, mB, p));
     SSDNERF_LAUNCH_OK();
     return 0;
 }
@@ -300,38 +236,7 @@ int conv_row2_launch(const ssdnerf_gemm_args* a, int sms, cudaStream_t stream) {
     CUtensorMap mB;
     if (int e = make_map_4d_box(&mB, a->b, ktot, a->n_rows_b ? a->n_rows_b : a->n, a->bx2 ? a->bx2 : 1, a->bx3 ? a->bx3 : 1, a->b_strides[0],
                                 a->b_strides[1], a->b_strides[2], kRwN, 1, 1)) return e;
-    return launch_row2<false>(mB, p, sms, stream);
+    return launch_row2(mB, p, sms, stream);
 }
 
 }  // namespace ssdnerf
-
-using namespace ssdnerf;
-
-extern "C" int ssdnerf_conv3x3_gn_f16(const ssdnerf_conv_gn_args* a, void* stream_) {
-    cudaStream_t stream = (cudaStream_t)stream_;
-    if (!a || !a->x1 || !a->q1 || !a->gamma || !a->beta || !a->w || !a->out || !a->coef_workspace)
-        return set_error_msg(SSDNERF_ERR_ARG, "conv3x3_gn: x1, q1, gamma, beta, w, out and coef_workspace are required");
-    if (a->B == 0 || a->H == 0) return 0;
-    if (a->H % 2) return set_error_msg(SSDNERF_ERR_ARG, "conv3x3_gn: H must be even (tiles are row pairs)");
-    if (a->C1 == 0 || a->C1 % 64 || a->C2 % 64 || (a->x2 && !a->q2)) return set_error_msg(SSDNERF_ERR_ARG, "conv3x3_gn: channel counts must be multiples of 64; x2 needs q2");
-    const uint32_t C = a->C1 + (a->x2 ? a->C2 : 0);
-    if (C > (uint32_t)kGnMaxC || (C / 32) % 4) return set_error_msg(SSDNERF_ERR_ARG, "conv3x3_gn: at most 384 input channels, channels per group a multiple of 4");
-    if (a->w_rows < 128) return set_error_msg(SSDNERF_ERR_ARG, "conv3x3_gn: packed weight needs >= 128 rows per tap");
-    if (((uintptr_t)a->x1 | (uintptr_t)a->x2 | (uintptr_t)a->out | (uintptr_t)a->residual | (uintptr_t)a->w | (uintptr_t)a->coef_workspace) & 15u)
-        return set_error_msg(SSDNERF_ERR_ARG, "conv3x3_gn: tensors must be 16-byte aligned");
-    ConvRowParams p{};
-    p.B = a->B; p.H = a->H; p.x1 = (const __half*)a->x1; p.C1 = a->C1; p.x2 = (const __half*)a->x2; p.C2 = a->x2 ? a->C2 : 0;
-    p.xs1[0] = p.C1; p.xs1[1] = (long long)kRwW * p.C1; p.xs1[2] = (long long)p.H * kRwW * p.C1;
-    p.xs2[0] = p.C2; p.xs2[1] = (long long)kRwW * p.C2; p.xs2[2] = (long long)p.H * kRwW * p.C2;
-    p.coef = (const float2*)a->coef_workspace; p.bias = a->bias; p.residual = (const __half*)a->residual; p.out = (__half*)a->out; p.qstats = a->qstats;
-    int dev = 0, sms = 0;
-    SSDNERF_CUDA_OK(cudaGetDevice(&dev));
-    SSDNERF_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    SSDNERF_CUDA_OK(launch_pdl(k_gn_coef, dim3(a->B), dim3(128), 0, stream, a->q1, a->C1, a->x2 ? a->q2 : (const float*)nullptr, p.C2, a->H * 128u,
-                               a->gamma, a->beta, a->scale_shift, a->ss_batch_stride, a->eps, (float2*)a->coef_workspace));
-    SSDNERF_LAUNCH_OK();
-    CUtensorMap mB;
-    if (int e = make_map_4d_box(&mB, a->w, C, a->w_rows, 9, 1, (uint64_t)C * 2, (uint64_t)a->w_rows * C * 2, (uint64_t)9 * a->w_rows * C * 2,
-                                kRwN, 1, 1)) return e;
-    return launch_row2<true>(mB, p, sms, stream);
-}

@@ -26,7 +26,7 @@ int set_error_msg(int code, const char* msg) {
 
 extern "C" {
 const char* ssdnerf_last_error(void) { return ssdnerf::g_err; }
-int ssdnerf_version(void) { return 100; }
+int ssdnerf_version(void) { return 101; }
 int ssdnerf_compiled_arch(void) { return 90; }
 unsigned long long ssdnerf_launch_count(void) { return __atomic_load_n(&ssdnerf::g_launches, __ATOMIC_RELAXED); }
 }

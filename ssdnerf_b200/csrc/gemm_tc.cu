@@ -11,7 +11,6 @@
 //   64 x BN fp32 in registers with wgmma.mma_async (m64nBNk16, fp16 x fp16 -> fp32, both operands from shared memory), then runs the
 //   epilogue (bias / residual / GroupNorm quad statistics / store) straight from the accumulator fragments while the producer already
 //   fills the stages of the next tile.
-// * clusters of CL = 2 / 4 / 8 CTAs along M: each CTA fetches 1/CL of the B (weight) tile and TMA-multicasts it to the whole cluster.
 // * narrow-channel family (KT = true, algo 3; the tiled-triplane UNet's 80 / 160 / 320 channels and 40 / 80-wide attention heads):
 //   K extents per source are multiples of 8 instead of 64.  A source's last 64-wide K chunk is a short slab: TMA zero-fills the box
 //   beyond the tensor map's K extent and the consumers issue only the ceil(valid / 16) k-steps that hold data.  The N tile is one of
@@ -54,16 +53,12 @@ struct GemmParams {
     long long so1, so2, so3;    // output element strides of d1, d2, d3 (column stride 1)
     float* qstats;              // optional [images][n_valid/4][2]: per-image sum / sum-of-squares of every 4-channel quad of the output
     uint32_t stats_hw;          // > 0: image index of a row = (row index along d1) / stats_hw; 0: image index = index along d3
-    unsigned long long* prof;   // optional debug counters (clock cycles summed over CTAs): [0] producer wait-empty, [1] producer total,
-                                // [2] consumer wait-full (warpgroup 1), [4] consumer total (warpgroup 1)
     uint32_t k1, k2;            // narrow family only: K elements per tap of A1 / A2 (the B operand holds them back to back)
 };
 
-// CL = cluster size: 1 = single CTA; 2 / 4 / 8 = multicast cluster (every CTA loads 1/CL of the B tile and multicasts it to all)
-template <int BN, int CL>
+template <int BN>
 struct GemmCfg {
     static constexpr int kBBytes = BN * kBK * 2;
-    static constexpr int kBoxRowsB = BN / CL;                // B rows fetched by ONE TMA instruction of this CTA
     static constexpr int kStageBytes = kABytes + kBBytes;
     static constexpr int kStages = (192 * 1024 / kStageBytes) > 8 ? 8 : (192 * 1024 / kStageBytes);
     static constexpr size_t kSmem = (size_t)kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/ + 1024 /*quad-stat accumulators*/ +
@@ -71,13 +66,12 @@ struct GemmCfg {
 };
 
 // The large layers are bound by operand delivery (L2 -> shared memory) rather than by the tensor cores: a 128 x BN tile re-fetches
-// (128 + BN) x 128 B per 64-wide k-block.  Wide N tiles (BN = 256, two consumer warpgroups of 64 x 256) amortise the A tile best;
-// multicast clusters additionally cut the B (weight) traffic by CL.
-template <int BN, int CL, bool KT>
+// (128 + BN) x 128 B per 64-wide k-block.  Wide N tiles (BN = 256, two consumer warpgroups of 64 x 256) amortise the A tile best.
+template <int BN, bool KT>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 k_gemm_tc(const __grid_constant__ CUtensorMap mapA1, const __grid_constant__ CUtensorMap mapA2,
           const __grid_constant__ CUtensorMap mapB, const GemmParams p) {
-    using Cfg = GemmCfg<BN, CL>;
+    using Cfg = GemmCfg<BN>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     uint8_t* sA = smem;
@@ -89,24 +83,20 @@ k_gemm_tc(const __grid_constant__ CUtensorMap mapA1, const __grid_constant__ CUt
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
     const uint32_t tiles_m = p.T1 * p.T2 * p.T3;
-    const uint32_t sup_m = (tiles_m + CL - 1) / CL;                 // super-tiles (CL M tiles) along M
-    const uint32_t total_tiles = sup_m * p.tiles_n;                   // work items per cluster
+    const uint32_t total_tiles = tiles_m * p.tiles_n;
     const uint32_t iters = p.taps * (p.kc1 + p.kc2);
-    const uint32_t crank = (CL > 1) ? cluster_ctarank() : 0u;
-    const uint32_t tile0 = (CL > 1) ? cluster_id_x() : blockIdx.x;
-    const uint32_t tile_step = (CL > 1) ? num_clusters_x() : gridDim.x;
-    constexpr uint16_t kMask = (uint16_t)((1u << CL) - 1u);
+    const uint32_t tile0 = blockIdx.x;
+    const uint32_t tile_step = gridDim.x;
 
     if (threadIdx.x == 0) {
         prefetch_tmap(&mapA1); prefetch_tmap(&mapA2); prefetch_tmap(&mapB);
-        // every consumer warp of every CTA of the cluster releases a stage (the multicast B slices land in all of them)
-        for (int i = 0; i < Cfg::kStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 8 * CL); }
+        // every consumer warp releases a stage
+        for (int i = 0; i < Cfg::kStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 8); }
         fence_mbar_init();
     }
     for (int i = threadIdx.x; i < BN; i += kGemmThreads) qacc[i] = 0.0f;     // 2 * BN/4 * 2 floats
     if (p.bias_n) for (uint32_t i = threadIdx.x; i < p.n_valid; i += kGemmThreads) sbias[i] = __ldg(p.bias_n + i);
     __syncthreads();
-    if (CL > 1) cluster_sync_all();       // peers' barriers are initialised before any multicast load / remote arrive targets them
     // everything above touched only shared memory and constant weights (bias): it may overlap the tail of the preceding kernel;
     // activations, residual, statistics and the output buffer are only touched after the dependency is resolved
     pdl_trigger();
@@ -117,15 +107,13 @@ k_gemm_tc(const __grid_constant__ CUtensorMap mapA1, const __grid_constant__ CUt
         setmaxnreg_dec<40>();
         if (threadIdx.x == 0) {   // ---------------- TMA producer
             uint32_t stage = 0, phase = 0;
-            long long pw = 0; const long long pt0 = clock64();
             for (uint32_t tile = tile0; tile < total_tiles; tile += tile_step) {
-                const uint32_t m_tile = (tile % sup_m) * CL + crank, n_tile = tile / sup_m;     // m_tile may be >= tiles_m in the last
-                const uint32_t t1 = m_tile % p.T1, t2 = (m_tile / p.T1) % p.T2, t3 = m_tile / (p.T1 * p.T2);   // super-tile: loads zero-fill
+                const uint32_t m_tile = tile % tiles_m, n_tile = tile / tiles_m;
+                const uint32_t t1 = m_tile % p.T1, t2 = (m_tile / p.T1) % p.T2, t3 = m_tile / (p.T1 * p.T2);
                 for (uint32_t tap = 0; tap < p.taps; ++tap) {
                     const int ox = p.tap_ox[tap], oy = p.tap_oy[tap];
                     for (uint32_t j = 0; j < p.kc1 + p.kc2; ++j) {
-                        if (p.prof) { const long long c = clock64(); mbar_wait(&empty[stage], phase ^ 1); pw += clock64() - c; }
-                        else mbar_wait(&empty[stage], phase ^ 1);
+                        mbar_wait(&empty[stage], phase ^ 1);
                         const bool first = j < p.kc1;
                         const int ak = (int)((first ? j : j - p.kc1) * kBK), a1 = (int)(t1 * p.b1 * p.a_stride) + ox, a2 = (int)(t2 * p.b2 * p.a_stride) + oy, a3 = (int)(t3 * p.b3);
                         mbar_expect_tx(&full[stage], (uint32_t)Cfg::kStageBytes);     // zero-filled box elements count too
@@ -133,18 +121,12 @@ k_gemm_tc(const __grid_constant__ CUtensorMap mapA1, const __grid_constant__ CUt
                         // B holds the two sources' K ranges back to back: with 64-aligned extents that is chunk j * 64, a short first
                         // source shifts the second one's chunks to k1 + (j - kc1) * 64
                         const int bk = KT ? (first ? ak : (int)p.k1 + ak) : (int)(j * kBK);
-                        if (CL == 1) {
-                            tma_load_4d(sB + stage * Cfg::kBBytes, &mapB, &full[stage], bk, (int)(n_tile * BN),
-                                        p.b_batched ? (int)t2 : (int)tap, p.b_batched ? (int)t3 : 0);
-                        } else {   // this CTA's 1/CL slice of the B tile, broadcast to the whole cluster
-                            tma_load_4d_mc(sB + stage * Cfg::kBBytes + crank * Cfg::kBoxRowsB * 128, &mapB, &full[stage], (int)(j * kBK),
-                                           (int)(n_tile * BN + crank * Cfg::kBoxRowsB), (int)tap, 0, kMask);
-                        }
+                        tma_load_4d(sB + stage * Cfg::kBBytes, &mapB, &full[stage], bk, (int)(n_tile * BN),
+                                    p.b_batched ? (int)t2 : (int)tap, p.b_batched ? (int)t3 : 0);
                         if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
                     }
                 }
             }
-            if (p.prof) { atomicAdd(p.prof + 0, (unsigned long long)pw); atomicAdd(p.prof + 1, (unsigned long long)(clock64() - pt0)); }
         }
     } else {   // ---------------- consumers: warpgroup cw owns rows 64 cw .. 64 cw + 63 of every tile
         setmaxnreg_inc<232>();
@@ -153,24 +135,17 @@ k_gemm_tc(const __grid_constant__ CUtensorMap mapA1, const __grid_constant__ CUt
         const uint32_t rbase = cw * 64u + wq * 16u + ((uint32_t)lane >> 2);     // this thread's rows: rbase, rbase + 8
         const uint32_t cq = (uint32_t)lane & 3u;
         uint32_t stage = 0, phase = 0;
-        long long wf = 0; const long long ct0 = clock64();
         float acc[BN / 2];
-        auto release = [&](uint32_t s) {
-            if (lane == 0) {
-                if (CL == 1) mbar_arrive(&empty[s]);
-                else for (uint32_t r = 0; r < (uint32_t)CL; ++r) mbar_arrive_cluster(mapa_u32(smem_u32(&empty[s]), r));
-            }
-        };
+        auto release = [&](uint32_t s) { if (lane == 0) mbar_arrive(&empty[s]); };
         for (uint32_t tile = tile0; tile < total_tiles; tile += tile_step) {
-            const uint32_t m_tile = (tile % sup_m) * CL + crank, n_tile = tile / sup_m;
+            const uint32_t m_tile = tile % tiles_m, n_tile = tile / tiles_m;
             const uint32_t t1 = m_tile % p.T1, t2 = (m_tile / p.T1) % p.T2, t3 = m_tile / (p.T1 * p.T2);
 #pragma unroll
             for (int i = 0; i < BN / 2; ++i) acc[i] = 0.0f;
             uint32_t prev = 0;
             uint32_t jc = 0;                              // KT: chunk index within the current tap
             for (uint32_t it = 0; it < iters; ++it) {
-                if (p.prof && cw == 0) { const long long c = clock64(); mbar_wait(&full[stage], phase); wf += clock64() - c; }
-                else mbar_wait(&full[stage], phase);
+                mbar_wait(&full[stage], phase);
                 const uint64_t a_desc = make_desc_sw128(smem_u32(sA + stage * kABytes + cw * 64 * 128));
                 const uint64_t b_desc = make_desc_sw128(smem_u32(sB + stage * Cfg::kBBytes));
                 wgmma_fence();
@@ -278,10 +253,8 @@ k_gemm_tc(const __grid_constant__ CUtensorMap mapA1, const __grid_constant__ CUt
                 asm volatile("bar.sync 1, 256;" ::: "memory");
             }
         }
-        if (p.prof && threadIdx.x == 128) { atomicAdd(p.prof + 2, (unsigned long long)wf); atomicAdd(p.prof + 4, (unsigned long long)(clock64() - ct0)); }
     }
     __syncthreads();
-    if (CL > 1) cluster_sync_all();       // nobody exits while a peer may still multicast into its shared memory or arrive on its barriers
 }
 
 // ---------------------------------------------------------------- host side: tensor maps
@@ -330,43 +303,25 @@ int make_map_4d_box(CUtensorMap* m, const void* base, uint64_t K, uint64_t e1, u
 }
 int conv_row2_launch(const ssdnerf_gemm_args* a, int sms, cudaStream_t stream);   // conv_row2.cu
 
-template <int BN, int CL, bool KT = false>
+template <int BN, bool KT = false>
 static int launch_gemm(const CUtensorMap& mA1, const CUtensorMap& mA2, const CUtensorMap& mB, const GemmParams& p, int sms,
                        cudaStream_t stream) {
-    using Cfg = GemmCfg<BN, CL>;
+    using Cfg = GemmCfg<BN>;
     static DeviceOnce attr;
     if (attr.first()) {
-        SSDNERF_CUDA_OK(cudaFuncSetAttribute(k_gemm_tc<BN, CL, KT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::kSmem));
+        SSDNERF_CUDA_OK(cudaFuncSetAttribute(k_gemm_tc<BN, KT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::kSmem));
     }
-    const uint32_t tiles_m = p.T1 * p.T2 * p.T3;
-    const uint32_t total = ((tiles_m + CL - 1) / CL) * p.tiles_n;          // work items per cluster (CL = 1: per CTA)
+    const uint32_t total = p.T1 * p.T2 * p.T3 * p.tiles_n;
     cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(total < (uint32_t)sms ? total : (uint32_t)sms);
     cfg.blockDim = dim3(kGemmThreads);
     cfg.dynamicSmemBytes = Cfg::kSmem;
     cfg.stream = stream;
-    cudaLaunchAttribute at[2];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = CL; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[1].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-    cfg.attrs = at; cfg.numAttrs = 2;
-    static int max_clusters_dev[64] = {};     // co-resident clusters of this instantiation (1 CTA / SM; GPC sizes limit clusters)
-    int& max_clusters_cached = max_clusters_dev[current_device()];
-    if (!max_clusters_cached) {
-        max_clusters_cached = sms / CL;
-        if (CL > 1) {
-            cfg.gridDim = dim3((uint32_t)(sms / CL) * CL);
-            int n = 0;
-            cfg.numAttrs = 1;
-            if (cudaOccupancyMaxActiveClusters(&n, k_gemm_tc<BN, CL, KT>, &cfg) == cudaSuccess && n > 0 && n < max_clusters_cached) max_clusters_cached = n;
-            cfg.numAttrs = 2;
-            (void)cudaGetLastError();
-        }
-    }
-    const uint32_t max_clusters = (uint32_t)max_clusters_cached;
-    const uint32_t clusters = total < max_clusters ? total : max_clusters;
-    cfg.gridDim = dim3(clusters * CL);
-    SSDNERF_CUDA_OK(cudaLaunchKernelEx(&cfg, k_gemm_tc<BN, CL, KT>, mA1, mA2, mB, p));
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
+    cfg.attrs = at; cfg.numAttrs = 1;
+    SSDNERF_CUDA_OK(cudaLaunchKernelEx(&cfg, k_gemm_tc<BN, KT>, mA1, mA2, mB, p));
     SSDNERF_LAUNCH_OK();
     return 0;
 }
@@ -383,7 +338,6 @@ extern "C" int ssdnerf_gemm_f16(const ssdnerf_gemm_args* a, void* stream_) {
     if (kt) {
         if (a->k1 == 0 || a->k1 % 8 || (a->a2 && (a->k2 == 0 || a->k2 % 8)))
             return set_error_msg(SSDNERF_ERR_ARG, "gemm (narrow): K extents must be multiples of 8");
-        if (a->cluster > 1) return set_error_msg(SSDNERF_ERR_ARG, "gemm (narrow): clusters are not built");
     } else if (a->k1 == 0 || a->k1 % 64 || a->k2 % 64) {
         return set_error_msg(SSDNERF_ERR_ARG, "gemm: K extents must be multiples of 64");
     }
@@ -400,7 +354,7 @@ extern "C" int ssdnerf_gemm_f16(const ssdnerf_gemm_args* a, void* stream_) {
     SSDNERF_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     // 3x3 convolution over 128-pixel rows with 128 output channels (the UNet's 128 x 128 level): row-pair kernel with halo reuse
     if (a->algo != 1 && !kt && a->taps == 9 && !a->tap_offsets && a_stride == 1 && a->d1 == 128 && a->b1 == 128 && a->b2 == 1 && a->b3 == 1 && a->n == 128 && !a->out_f32 && !a->b_batched &&
-        (a->d2 % 2) == 0 && a->alpha == 1.0f && (a->bn == 0 || a->bn == 128) && a->cluster <= 1 && a->so1 == 128 && a->so2 == 128 * 128 &&
+        (a->d2 % 2) == 0 && a->alpha == 1.0f && (a->bn == 0 || a->bn == 128) && a->so1 == 128 && a->so2 == 128 * 128 &&
         a->so3 == (long long)a->d2 * 128 * 128 && (!a->qstats || a->stats_hw == 0) && (a->n_rows_b == 0 || a->n_rows_b >= 128))
         return ssdnerf::conv_row2_launch(a, sms, stream);
     if (a->algo == 2) return set_error_msg(SSDNERF_ERR_ARG, "gemm: algo 2 (row-pair convolution) needs taps 9, 128-pixel rows, 128 output channels, fp16 output");
@@ -449,7 +403,7 @@ extern "C" int ssdnerf_gemm_f16(const ssdnerf_gemm_args* a, void* stream_) {
     p.k1 = a->k1; p.k2 = a->a2 ? a->k2 : 0; p.n_valid = a->n; p.b_batched = a->b_batched;
     p.alpha = a->alpha; p.bias_n = a->bias_n; p.residual = (const __half*)a->residual; p.out = a->out; p.out_f32 = a->out_f32;
     p.so1 = a->so1; p.so2 = a->so2; p.so3 = a->so3;
-    p.qstats = a->qstats; p.stats_hw = a->stats_hw; p.prof = (unsigned long long*)a->debug_cycles;
+    p.qstats = a->qstats; p.stats_hw = a->stats_hw;
     // element pairs (2 n, 2 n + 1) of a row are stored / read as one 4-byte (fp16) or 8-byte (fp32) access when every row offset is even
     const uintptr_t pair_align = a->out_f32 ? 8u : 4u;
     p.vec2 = ((a->so1 | a->so2 | a->so3) & 1) == 0 && ((uintptr_t)a->out % pair_align) == 0 && ((uintptr_t)a->residual & 3u) == 0;
@@ -468,33 +422,21 @@ extern "C" int ssdnerf_gemm_f16(const ssdnerf_gemm_args* a, void* stream_) {
     } else {
         mA2 = mA1;
     }
-    // clusters along M (weights shared, multicast B slices): only for non-batched B and on request; multicast cuts L2 traffic but not
-    // the staged bytes per SM, so auto stays with single CTAs
-    int cl = 1;
-    if ((a->cluster == 2 || a->cluster == 4 || a->cluster == 8) && !a->b_batched && bn >= 128) cl = (int)a->cluster;
-    // B: {K, N, x2, x3}; box {64, rows fetched per TMA instruction (bn: single CTA, bn / cl: multicast slice), 1, 1}
+    // B: {K, N, x2, x3}; box {64, bn, 1, 1}
     if (int e = make_map_4d(&mB, a->b, ktot, a->n_rows_b ? a->n_rows_b : a->n, a->bx2 ? a->bx2 : 1, a->bx3 ? a->bx3 : 1, a->b_strides[0],
-                            a->b_strides[1], a->b_strides[2], (uint32_t)(bn / cl), 1, 1)) return e;
+                            a->b_strides[1], a->b_strides[2], (uint32_t)bn, 1, 1)) return e;
 
     if (kt) {
         switch (bn) {
-            case 256: return launch_gemm<256, 1, true>(mA1, mA2, mB, p, sms, stream);
-            case 160: return launch_gemm<160, 1, true>(mA1, mA2, mB, p, sms, stream);
-            case 80: return launch_gemm<80, 1, true>(mA1, mA2, mB, p, sms, stream);
-            case 48: return launch_gemm<48, 1, true>(mA1, mA2, mB, p, sms, stream);
-            case 40: return launch_gemm<40, 1, true>(mA1, mA2, mB, p, sms, stream);
-            default: return launch_gemm<16, 1, true>(mA1, mA2, mB, p, sms, stream);
+            case 256: return launch_gemm<256, true>(mA1, mA2, mB, p, sms, stream);
+            case 160: return launch_gemm<160, true>(mA1, mA2, mB, p, sms, stream);
+            case 80: return launch_gemm<80, true>(mA1, mA2, mB, p, sms, stream);
+            case 48: return launch_gemm<48, true>(mA1, mA2, mB, p, sms, stream);
+            case 40: return launch_gemm<40, true>(mA1, mA2, mB, p, sms, stream);
+            default: return launch_gemm<16, true>(mA1, mA2, mB, p, sms, stream);
         }
     }
-    if (bn == 256) {
-        if (cl == 8) return launch_gemm<256, 8>(mA1, mA2, mB, p, sms, stream);
-        if (cl == 4) return launch_gemm<256, 4>(mA1, mA2, mB, p, sms, stream);
-        return cl == 2 ? launch_gemm<256, 2>(mA1, mA2, mB, p, sms, stream) : launch_gemm<256, 1>(mA1, mA2, mB, p, sms, stream);
-    }
-    if (bn == 128) {
-        if (cl == 8) return launch_gemm<128, 8>(mA1, mA2, mB, p, sms, stream);
-        if (cl == 4) return launch_gemm<128, 4>(mA1, mA2, mB, p, sms, stream);
-        return cl == 2 ? launch_gemm<128, 2>(mA1, mA2, mB, p, sms, stream) : launch_gemm<128, 1>(mA1, mA2, mB, p, sms, stream);
-    }
-    return launch_gemm<64, 1>(mA1, mA2, mB, p, sms, stream);
+    if (bn == 256) return launch_gemm<256>(mA1, mA2, mB, p, sms, stream);
+    if (bn == 128) return launch_gemm<128>(mA1, mA2, mB, p, sms, stream);
+    return launch_gemm<64>(mA1, mA2, mB, p, sms, stream);
 }

@@ -171,41 +171,6 @@ __global__ void __launch_bounds__(256) k_gn_apply(const __half* __restrict__ x1,
     for (; p < p1; p += pstep) emit(__ldg(reinterpret_cast<const uint4*>(src + (size_t)p * cs)), p);
 }
 
-// ---------------------------------------------------------------- stride-2 3x3 im2col: [B,H,W,C] -> [B,H/2,W/2,9C]
-__global__ void k_im2col_s2(const __half* __restrict__ x, uint32_t B, uint32_t H, uint32_t W, uint32_t C, __half* __restrict__ out) {
-    pdl_trigger();
-    pdl_wait();
-    const uint32_t cv = C / 8, Ho = H / 2, Wo = W / 2;
-    const size_t i = threadIdx.x + (size_t)blockIdx.x * blockDim.x;   // over B*Ho*Wo*9*cv
-    if (i >= (size_t)B * Ho * Wo * 9 * cv) return;
-    const uint32_t v = (uint32_t)(i % cv);
-    size_t r = i / cv;
-    const uint32_t tap = (uint32_t)(r % 9); r /= 9;
-    const uint32_t ox = (uint32_t)(r % Wo); r /= Wo;
-    const uint32_t oy = (uint32_t)(r % Ho);
-    const uint32_t b = (uint32_t)(r / Ho);
-    const int iy = 2 * (int)oy + (int)(tap / 3) - 1, ix = 2 * (int)ox + (int)(tap % 3) - 1;
-    uint4 val = make_uint4(0, 0, 0, 0);
-    if (iy >= 0 && iy < (int)H && ix >= 0 && ix < (int)W)
-        val = __ldg(reinterpret_cast<const uint4*>(x + (((size_t)b * H + iy) * W + ix) * C) + v);
-    reinterpret_cast<uint4*>(out)[i] = val;
-}
-
-// ---------------------------------------------------------------- nearest x2: [B,H,W,C] -> [B,2H,2W,C]
-__global__ void k_upsample2x(const __half* __restrict__ x, uint32_t B, uint32_t H, uint32_t W, uint32_t C, __half* __restrict__ out) {
-    pdl_trigger();
-    pdl_wait();
-    const uint32_t cv = C / 8;
-    const size_t i = threadIdx.x + (size_t)blockIdx.x * blockDim.x;   // over B*2H*2W*cv
-    if (i >= (size_t)B * 4 * H * W * cv) return;
-    const uint32_t v = (uint32_t)(i % cv);
-    size_t r = i / cv;
-    const uint32_t ox = (uint32_t)(r % (2 * W)); r /= 2 * W;
-    const uint32_t oy = (uint32_t)(r % (2 * H));
-    const uint32_t b = (uint32_t)(r / (2 * H));
-    reinterpret_cast<uint4*>(out)[i] = __ldg(reinterpret_cast<const uint4*>(x + (((size_t)b * H + oy / 2) * W + ox / 2) * C) + v);
-}
-
 // ---------------------------------------------------------------- softmax over rows of fp32 S [rows][T] -> fp16 P
 __global__ void __launch_bounds__(256) k_softmax_rows(const float* __restrict__ S, uint32_t rows, uint32_t T, __half* __restrict__ P) {
     pdl_trigger();
@@ -376,26 +341,6 @@ int ssdnerf_gn_apply_q(const void* x1, uint32_t C1, const void* x2, uint32_t C2,
         return set_error_msg(SSDNERF_ERR_ARG, "gn_apply_q: channels per group and per source must be multiples of 4");
     if (!q1 || (x2 && !q2)) return set_error_msg(SSDNERF_ERR_ARG, "gn_apply_q: quad statistics missing");
     return gn_apply_impl(x1, C1, x2, C2, B, HW, groups, q1, q2, 1, gamma, beta, scale_shift, ss_batch_stride, eps, do_silu, out, stream);
-}
-
-int ssdnerf_im2col_s2(const void* x, uint32_t B, uint32_t H, uint32_t W, uint32_t C, void* out, void* stream) {
-    if (C % 8 || H % 2 || W % 2) return set_error_msg(SSDNERF_ERR_ARG, "im2col_s2: C % 8, H % 2, W % 2 must be 0");
-    CHK_ALIGN16(x, "im2col_s2"); CHK_ALIGN16(out, "im2col_s2");
-    const size_t n = (size_t)B * (H / 2) * (W / 2) * 9 * (C / 8);
-    if (!n) return 0;
-    SSDNERF_CUDA_OK(launch_pdl(k_im2col_s2, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, (const __half*)x, B, H, W, C, (__half*)out));
-    SSDNERF_LAUNCH_OK();
-    return 0;
-}
-
-int ssdnerf_upsample2x(const void* x, uint32_t B, uint32_t H, uint32_t W, uint32_t C, void* out, void* stream) {
-    if (C % 8) return set_error_msg(SSDNERF_ERR_ARG, "upsample2x: C % 8 must be 0");
-    CHK_ALIGN16(x, "upsample2x"); CHK_ALIGN16(out, "upsample2x");
-    const size_t n = (size_t)B * 4 * H * W * (C / 8);
-    if (!n) return 0;
-    SSDNERF_CUDA_OK(launch_pdl(k_upsample2x, dim3(blocks_for(n, 256)), dim3(256), 0, (cudaStream_t)stream, (const __half*)x, B, H, W, C, (__half*)out));
-    SSDNERF_LAUNCH_OK();
-    return 0;
 }
 
 int ssdnerf_softmax_rows(const float* S, uint32_t rows, uint32_t T, void* P, void* stream) {

@@ -9,7 +9,6 @@ softmax and layout glue as fused memory-bound kernels.  Forward semantics of the
 mmgen 0.7.2 are restated per SURVEY.md Appendix B.  Inference only (no autograd through the engine).
 """
 import math
-import os
 from copy import deepcopy
 
 import torch
@@ -283,10 +282,6 @@ class UNetEngine:
         if any(c % m.num_heads or (c // m.num_heads) % 8 for c in attn_widths):
             raise NotImplementedError(f'native UNet engine: attention head widths must be multiples of 8; got widths {attn_widths} over '
                                       f'{m.num_heads} heads')
-        self.flash_attention = True      # False: unfused scores -> softmax -> PV composition (A/B tests)
-        # 128x128-level resblocks: GroupNorm + SiLU inside the row-pair conv kernel (csrc/conv_row2.cu).  Opt-in (SSDNERF_FUSED_GN_CONV=1):
-        # the default is the GroupNorm-apply pass followed by the row-pair convolution
-        self.fused_gn_conv = os.environ.get('SSDNERF_FUSED_GN_CONV', '0') == '1'
         self.H, self.W = (int(v) for v in (hw if hw is not None else m.image_size))
         self.bufs = {}
         self.cin_total = m.in_channels + m.concat_cond_channels
@@ -444,31 +439,20 @@ class UNetEngine:
             sc = x
         qh1 = self._q(('h1', tag), cout)
         qo = self._q(('res_out', tag), cout)
-        if self.saving:       # keep what the input-gradient pass re-reads: raw inputs of both GroupNorms + their statistics
-            a = self._gn(x, qx, sk, qs, d['g1'], d['b1'], self._buf(('a', H, cin), (B, H, W, cin)), True)
-            st1 = self._last_stats
-            h1 = U.conv3x3_f16(a, d['w1'], cout, bias=d['c1b'], out=self._buf(('h1', tag), (B, H, W, cout)), qstats=qh1, narrow=nw)
-            a2 = self._gn(h1, qh1, None, None, d['g2'], d['b2'], self._buf(('a2', H, cout), (B, H, W, cout)), True, self.ss_offsets[d['idx']])
-            st2 = self._last_stats
-            self._dropout(a2, d['idx'])
-            out = U.conv3x3_f16(a2, d['w2'], cout, bias=d['c2b'], residual=sc, out=self._buf(('res_out', tag), (B, H, W, cout)), qstats=qo,
-                                narrow=nw)
-            self.tape.append(dict(kind='res', d=d, x=x, sk=sk, st1=st1, h1=h1, st2=st2, out=out, tag=tag))
-            return out, qo
-        if self.fused_gn_conv and not nw and self.groups == 32 and W == 128 and cout == 128 and cin <= 384 and (cin // 32) % 4 == 0:
-            # 128 x 128 level: GroupNorm apply + SiLU ride on the convolution's activation load path (csrc/conv_row2_gn.cu)
-            h1 = U.conv3x3_gn_f16(x, qx, d['g1'], d['b1'], d['w1'], bias=d['c1b'], x2=sk, q2=qs,
-                                  out=self._buf(('h1', H, cout), (B, H, W, cout)), qstats=qh1,
-                                  coef_ws=self._buf(('gncoef', 1, tag), (B * cin * 2,), torch.float32))
-            ss = N.c_void_p(self.ss_cur.data_ptr() + 4 * self.ss_offsets[d['idx']])
-            return U.conv3x3_gn_f16(h1, qh1, d['g2'], d['b2'], d['w2'], bias=d['c2b'], scale_shift_ptr=ss, ss_batch_stride=self.ss_total,
-                                    residual=sc, out=self._buf(('res_out', tag), (B, H, W, cout)), qstats=qo,
-                                    coef_ws=self._buf(('gncoef', 2, tag), (B * cout * 2,), torch.float32)), qo
         a = self._gn(x, qx, sk, qs, d['g1'], d['b1'], self._buf(('a', H, cin), (B, H, W, cin)), True)
-        h1 = U.conv3x3_f16(a, d['w1'], cout, bias=d['c1b'], out=self._buf(('h1', H, cout), (B, H, W, cout)), qstats=qh1, narrow=nw)
+        st1 = self._last_stats
+        # saving keeps what the input-gradient pass re-reads (raw inputs of both GroupNorms + their statistics): h1 in a buffer of its own
+        h1 = U.conv3x3_f16(a, d['w1'], cout, bias=d['c1b'], out=self._buf(('h1', tag) if self.saving else ('h1', H, cout), (B, H, W, cout)),
+                           qstats=qh1, narrow=nw)
         a2 = self._gn(h1, qh1, None, None, d['g2'], d['b2'], self._buf(('a2', H, cout), (B, H, W, cout)), True, self.ss_offsets[d['idx']])
-        return U.conv3x3_f16(a2, d['w2'], cout, bias=d['c2b'], residual=sc, out=self._buf(('res_out', tag), (B, H, W, cout)), qstats=qo,
-                             narrow=nw), qo
+        st2 = self._last_stats
+        if self.saving:
+            self._dropout(a2, d['idx'])
+        out = U.conv3x3_f16(a2, d['w2'], cout, bias=d['c2b'], residual=sc, out=self._buf(('res_out', tag), (B, H, W, cout)), qstats=qo,
+                            narrow=nw)
+        if self.saving:
+            self.tape.append(dict(kind='res', d=d, x=x, sk=sk, st1=st1, h1=h1, st2=st2, out=out, tag=tag))
+        return out, qo
 
     def _attn(self, d, x, tag):
         x, qx = x
@@ -494,7 +478,7 @@ class UNetEngine:
         """softmax(q k^T / sqrt(ch)) v on the qkv projection [B*T, 3c] (legacy head layout) -> [B, T, c]"""
         ch = c // heads
         L, s = N.lib(), N.stream_ptr()
-        if self.flash_attention and ch in (64, 128) and T % 64 == 0:
+        if ch in (64, 128) and T % 64 == 0:
             return U.flash_attn(qkv.view(B, T, 3 * c), heads, 1.0 / math.sqrt(ch), out=self._buf(out_key, (B, T, c)))
         # unfused composition (scores -> softmax -> P V), kept for head widths / lengths the fused kernel does not cover
         S = U.attn_scores(qkv.view(B, T, 3 * c), heads, scale=1.0 / math.sqrt(ch), out=self._buf(('S', T), (B, heads, T, T), torch.float32),

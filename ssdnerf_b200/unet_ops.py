@@ -26,25 +26,17 @@ class GemmArgs(ctypes.Structure):
         ('taps', N.c_u32),
         ('b', N.c_void_p), ('b_strides', c_u64 * 3), ('n', N.c_u32), ('n_rows_b', N.c_u32), ('bx2', N.c_u32), ('bx3', N.c_u32),
         ('b_batched', N.c_u32),
-        ('bn', N.c_u32), ('cluster', N.c_u32), ('alpha', N.c_f32), ('bias_n', N.c_void_p), ('residual', N.c_void_p),
+        ('bn', N.c_u32), ('alpha', N.c_f32), ('bias_n', N.c_void_p), ('residual', N.c_void_p),
         ('out', N.c_void_p), ('out_f32', N.c_u32), ('so1', c_ll), ('so2', c_ll), ('so3', c_ll),
-        ('qstats', N.c_void_p), ('stats_hw', N.c_u32), ('debug_cycles', N.c_void_p), ('algo', N.c_u32),
+        ('qstats', N.c_void_p), ('stats_hw', N.c_u32), ('algo', N.c_u32),
         ('tap_offsets', N.c_void_p), ('a_stride', N.c_u32),
     ]
 
 
 ALGO_NARROW = 3     # ssdnerf_gemm_args.algo of the narrow-channel family
 
-GEMM_PROF = None    # set to a uint64[8] CUDA tensor to collect the generic GEMM kernel's pipeline wait cycles (debug, ssdnerf_gemm_args.debug_cycles)
-GEMM_LOG = None     # set to a list to record (M, N, K, taps, bn, cluster, batched, fused_stats) of every launch (profiling scripts)
-
 
 def _launch(a):
-    if GEMM_PROF is not None:
-        a.debug_cycles = GEMM_PROF.data_ptr()
-    if GEMM_LOG is not None:
-        GEMM_LOG.append(dict(M=int(a.d1) * int(a.d2) * int(a.d3), N=int(a.n), K=int(a.k1) + int(a.k2), taps=int(a.taps), bn=int(a.bn),
-                             cluster=int(a.cluster), batched=int(a.b_batched), qstats=bool(a.qstats), f32=int(a.out_f32)))
     N.check(N.lib().ssdnerf_gemm_f16(ctypes.byref(a), N.stream_ptr()))
 
 
@@ -76,7 +68,7 @@ def pack_conv_weight(w, cin_pad=None, narrow=False):
     return _pad_rows(wp).contiguous()
 
 
-def linear_f16(a, w, bias=None, residual=None, out=None, out_f32=False, alpha=1.0, bn=0, n=None, cluster=0, qstats=None, stats_hw=0, narrow=False):
+def linear_f16(a, w, bias=None, residual=None, out=None, out_f32=False, alpha=1.0, bn=0, n=None, qstats=None, stats_hw=0, narrow=False):
     """out[M, N] = alpha * a[M, K] @ w[N, K]^T + bias + residual.  a fp16 [M, K] (row stride may exceed K)."""
     N.require_cuda(a, w)
     M, K = a.shape
@@ -92,7 +84,7 @@ def linear_f16(a, w, bias=None, residual=None, out=None, out_f32=False, alpha=1.
     g.b, g.n, g.n_rows_b, g.bx2, g.bx3 = w.data_ptr(), n, w.shape[0], 1, 1
     ws = w.stride(0) * 2
     g.b_strides = (c_u64 * 3)(ws, ws * w.shape[0], ws * w.shape[0])
-    g.bn, g.alpha, g.cluster = bn, alpha, cluster
+    g.bn, g.alpha = bn, alpha
     g.bias_n = bias.data_ptr() if bias is not None else None
     g.residual = residual.data_ptr() if residual is not None else None
     g.out, g.out_f32 = out.data_ptr(), int(out.dtype == torch.float32)
@@ -130,8 +122,7 @@ def _conv_boxes_narrow(H, W):
     return bw, bh, 128 // (bw * bh)
 
 
-def conv3x3_f16(x, wp, cout, bias=None, x2=None, residual=None, out=None, out_f32=False, taps=9, bn=0, cluster=0, qstats=None, algo=0,
-                narrow=False):
+def conv3x3_f16(x, wp, cout, bias=None, x2=None, residual=None, out=None, out_f32=False, taps=9, bn=0, qstats=None, algo=0, narrow=False):
     """3x3 (taps=9, pad 1, stride 1) or 1x1 (taps=1) convolution over NHWC fp16 x [B,H,W,C1] (+ x2 [B,H,W,C2] concatenated
     along channels).  wp: packed weight [taps][Cout_pad][C1+C2].  narrow: C1 / C2 multiples of 8 (narrow-channel family)."""
     N.require_cuda(x, wp)
@@ -157,7 +148,7 @@ def conv3x3_f16(x, wp, cout, bias=None, x2=None, residual=None, out=None, out_f3
     rows = wp.shape[-2]
     g.b, g.n, g.n_rows_b, g.bx2, g.bx3 = wp.data_ptr(), cout, rows, taps, 1
     g.b_strides = (c_u64 * 3)(ktot * 2, rows * ktot * 2, taps * rows * ktot * 2)
-    g.bn, g.alpha, g.cluster, g.algo = bn, 1.0, cluster, algo
+    g.bn, g.alpha, g.algo = bn, 1.0, algo
     g.bias_n = bias.data_ptr() if bias is not None else None
     g.residual = residual.data_ptr() if residual is not None else None
     g.out, g.out_f32 = out.data_ptr(), int(out.dtype == torch.float32)
@@ -314,48 +305,6 @@ def flash_attn(qkv, heads, scale, out=None):
         out = torch.empty(B, T, c, dtype=torch.float16, device=qkv.device)
     N.check(N.lib().ssdnerf_flash_attn(N.ptr(qkv), N.c_u32(B), N.c_u32(T), N.c_u32(heads), N.c_u32(ch), N.c_f32(scale), N.ptr(out),
                                        N.stream_ptr()))
-    return out
-
-
-class ConvGnArgs(ctypes.Structure):
-    """mirror of `ssdnerf_conv_gn_args`"""
-    _fields_ = [
-        ('x1', N.c_void_p), ('C1', N.c_u32), ('x2', N.c_void_p), ('C2', N.c_u32), ('B', N.c_u32), ('H', N.c_u32),
-        ('q1', N.c_void_p), ('q2', N.c_void_p), ('gamma', N.c_void_p), ('beta', N.c_void_p), ('scale_shift', N.c_void_p),
-        ('ss_batch_stride', c_ll), ('eps', N.c_f32), ('w', N.c_void_p), ('w_rows', N.c_u32), ('bias', N.c_void_p),
-        ('residual', N.c_void_p), ('out', N.c_void_p), ('qstats', N.c_void_p), ('coef_workspace', N.c_void_p),
-    ]
-
-
-def conv3x3_gn_f16(x1, q1, gamma, beta, wp, bias=None, x2=None, q2=None, scale_shift_ptr=None, ss_batch_stride=0, eps=1e-5,
-                   residual=None, out=None, qstats=None, coef_ws=None):
-    """out = conv3x3(SiLU(GroupNorm32(cat(x1, x2)) * (1 + scale) + shift)) + bias + residual on RAW inputs (csrc/conv_row2_gn.cu).
-    x1 / x2 NHWC fp16 [B,H,128,C]; q1 / q2 their quad statistics; wp packed weight [9][rows][C1+C2]; 128 output channels."""
-    N.require_cuda(x1, wp, q1)
-    B, H, W, C1 = x1.shape
-    assert W == 128 and x1.is_contiguous() and (x2 is None or x2.is_contiguous())
-    if out is None:
-        out = torch.empty(B, H, W, 128, dtype=torch.float16, device=x1.device)
-    a = ConvGnArgs()
-    a.x1, a.C1 = x1.data_ptr(), C1
-    if x2 is not None:
-        a.x2, a.C2, a.q2 = x2.data_ptr(), x2.shape[-1], q2.data_ptr()
-    a.B, a.H = B, H
-    a.q1, a.gamma, a.beta = q1.data_ptr(), gamma.data_ptr(), beta.data_ptr()
-    if scale_shift_ptr is not None:
-        a.scale_shift, a.ss_batch_stride = scale_shift_ptr, ss_batch_stride
-    a.eps = eps
-    a.w, a.w_rows = wp.data_ptr(), wp.shape[-2]
-    a.bias = bias.data_ptr() if bias is not None else None
-    a.residual = residual.data_ptr() if residual is not None else None
-    a.out = out.data_ptr()
-    a.qstats = qstats.data_ptr() if qstats is not None else None
-    if coef_ws is None:
-        coef_ws = torch.empty(B * (C1 + (x2.shape[-1] if x2 is not None else 0)) * 2, dtype=torch.float32, device=x1.device)
-    a.coef_workspace = coef_ws.data_ptr()
-    if GEMM_LOG is not None:
-        GEMM_LOG.append(dict(M=B * H * W, N=128, K=int(a.C1) + int(a.C2), taps=9, bn=128, cluster=1, batched=0, qstats=bool(a.qstats), f32=0, fused_gn=True))
-    N.check(N.lib().ssdnerf_conv3x3_gn_f16(ctypes.byref(a), N.stream_ptr()))
     return out
 
 

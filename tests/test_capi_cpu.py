@@ -57,11 +57,13 @@ def test_unknown_decoder_variant_is_rejected_before_any_launch():
 
 
 def test_ctypes_arg_structs_match_header(tmp_path):
-    """RenderArgs / RenderTrainArgs mirror ssdnerf_render_args / ssdnerf_render_train_args field by field: the host compiler's
-    sizeof and offsetof for the header equal ctypes' layout"""
+    """every ctypes argument struct mirrors its header struct field by field: the host compiler's sizeof and offsetof for the header
+    equal ctypes' layout"""
     import subprocess
     from ssdnerf_b200 import _lib as N
-    mirrors = {'ssdnerf_render_args': N.RenderArgs, 'ssdnerf_render_train_args': N.RenderTrainArgs}
+    from ssdnerf_b200 import unet_ops as U
+    mirrors = {'ssdnerf_render_args': N.RenderArgs, 'ssdnerf_render_train_args': N.RenderTrainArgs, 'ssdnerf_gemm_args': U.GemmArgs,
+               'ssdnerf_gn_bwd_args': U.GnBwdArgs, 'ssdnerf_wgrad_args': U.WgradArgs}
     lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "ssdnerf_b200.h"', 'int main(void) {']
     expect = []
     for cname, mirror in mirrors.items():
