@@ -263,6 +263,8 @@ typedef struct ssdnerf_gemm_args {
      * a_stride 2 = stride-2 convolution: (d1, d2) are output extents, a1 / a2 describe the (2 d1 x 2 d2) input read at every 2nd pixel */
     const int8_t* tap_offsets;   /* HOST pointer, 2 * taps entries, or NULL */
     uint32_t a_stride;           /* 0 / 1: dense; 2: stride-2 convolution */
+    uint32_t relu;               /* 1: out = max(0, D + bias + residual) (default family, or the narrow family with its 16-column N tile);
+                                  * never takes the row-pair convolution */
 } ssdnerf_gemm_args;
 SSDNERF_API int ssdnerf_gemm_f16(const ssdnerf_gemm_args* args, void* stream);
 
@@ -371,6 +373,28 @@ SSDNERF_API int ssdnerf_conv_wgrad_f16(const ssdnerf_wgrad_args* args, void* str
  * replaces nn.Dropout of DenoisingResBlock (mmgen, used by lib/models/architecture/diffusion/modules.py:51-110) in training */
 SSDNERF_API int ssdnerf_dropout_f16(void* x, unsigned long long n, unsigned long long seed, float p_drop, void* stream);
 SSDNERF_API int ssdnerf_colsum_f16(const void* src, uint64_t rows, uint32_t stride, uint32_t c0, uint32_t channels, float* out, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * 5. Evaluation metrics of val_step: SSIM and the LPIPS(VGG16) stages around the convolutions.
+ *    replaces: skimage.metrics.structural_similarity and lpips.LPIPS(net='vgg') as called by
+ *              lib/core/evaluation/metrics.py:58-71 from lib/models/autodecoders/base_nerf.py:555-572.
+ *    Images are channels-last fp32 [n][h][w][3] in [0, 1], as the renderer writes them.
+ * ---------------------------------------------------------------------------------------------- */
+/* out[i] = SSIM(pred[i], target[i]) with skimage's defaults for channel_axis / data_range = 1: 7 x 7 uniform window, sample covariance,
+ * C1 = 0.01^2, C2 = 0.03^2, mean over the interior [3:h-3, 3:w-3] of each channel, then over the channels.  Moments in fp64, fixed-order
+ * per-image reduction (bit-identical run to run).  h, w >= 7 and w <= 1600, else SSDNERF_ERR_ARG. */
+SSDNERF_API int ssdnerf_ssim_f32(const float* pred, const float* target, uint32_t n, uint32_t h, uint32_t w, float* out, void* stream);
+/* LPIPS input: out fp16 [2m][h][w][16] = ((2 x - 1) - shift) / scale (lpips ScalingLayer) in channels 0..2, zeros above;
+ * images 0..m-1 from pred [m][h][w][3], m..2m-1 from target */
+SSDNERF_API int ssdnerf_lpips_prep_f16(const float* pred, const float* target, uint32_t m, uint32_t h, uint32_t w, void* out, void* stream);
+/* floats of the `partial` scratch ssdnerf_lpips_tap_f16 needs for these extents (0 for an unsupported channel count) */
+SSDNERF_API uint32_t ssdnerf_lpips_tap_partials(uint32_t m, uint32_t h, uint32_t w, uint32_t c, int pool);
+/* one LPIPS tap over the post-ReLU fp16 map feat [2m][h][w][c] (pred images first), c in {64, 128, 256, 512}:
+ *   out[j] += mean over pixels of sum_c lin[c] * (fp / (|fp| + 1e-10) - ft / (|ft| + 1e-10))^2, fp = feat[j], ft = feat[m + j]
+ * (per-pair partial sums in `partial`, then added in a fixed order); pooled != NULL (even h, w) also gets the 2 x 2 / 2 max-pooled map
+ * fp16 [2m][h/2][w/2][c] */
+SSDNERF_API int ssdnerf_lpips_tap_f16(const void* feat, uint32_t m, uint32_t h, uint32_t w, uint32_t c, const float* lin, float* partial,
+                                     void* pooled, float* out, void* stream);
 
 #ifdef __cplusplus
 }

@@ -67,7 +67,8 @@ struct GemmCfg {
 
 // The large layers are bound by operand delivery (L2 -> shared memory) rather than by the tensor cores: a 128 x BN tile re-fetches
 // (128 + BN) x 128 B per 64-wide k-block.  Wide N tiles (BN = 256, two consumer warpgroups of 64 x 256) amortise the A tile best.
-template <int BN, bool KT>
+// RELU: max(0, .) after bias / residual, before the store (LPIPS' VGG16 convolutions); its own instantiations, so the others are unchanged.
+template <int BN, bool KT, bool RELU = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 k_gemm_tc(const __grid_constant__ CUtensorMap mapA1, const __grid_constant__ CUtensorMap mapA2,
           const __grid_constant__ CUtensorMap mapB, const GemmParams p) {
@@ -219,6 +220,7 @@ k_gemm_tc(const __grid_constant__ CUtensorMap mapA1, const __grid_constant__ CUt
                             if (okc1) v1 += __half2float(p.residual[o + 1]);
                         }
                     }
+                    if constexpr (RELU) { v0 = fmaxf(v0, 0.0f); v1 = fmaxf(v1, 0.0f); }
                     if (p.out_f32) {
                         float* op = reinterpret_cast<float*>(p.out) + o;
                         if (p.vec2 && okc1) *reinterpret_cast<float2*>(op) = make_float2(v0, v1);
@@ -303,13 +305,13 @@ int make_map_4d_box(CUtensorMap* m, const void* base, uint64_t K, uint64_t e1, u
 }
 int conv_row2_launch(const ssdnerf_gemm_args* a, int sms, cudaStream_t stream);   // conv_row2.cu
 
-template <int BN, bool KT = false>
+template <int BN, bool KT = false, bool RELU = false>
 static int launch_gemm(const CUtensorMap& mA1, const CUtensorMap& mA2, const CUtensorMap& mB, const GemmParams& p, int sms,
                        cudaStream_t stream) {
     using Cfg = GemmCfg<BN>;
     static DeviceOnce attr;
     if (attr.first()) {
-        SSDNERF_CUDA_OK(cudaFuncSetAttribute(k_gemm_tc<BN, KT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::kSmem));
+        SSDNERF_CUDA_OK(cudaFuncSetAttribute(k_gemm_tc<BN, KT, RELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::kSmem));
     }
     const uint32_t total = p.T1 * p.T2 * p.T3 * p.tiles_n;
     cudaLaunchConfig_t cfg{};
@@ -321,7 +323,7 @@ static int launch_gemm(const CUtensorMap& mA1, const CUtensorMap& mA2, const CUt
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
     cfg.attrs = at; cfg.numAttrs = 1;
-    SSDNERF_CUDA_OK(cudaLaunchKernelEx(&cfg, k_gemm_tc<BN, KT>, mA1, mA2, mB, p));
+    SSDNERF_CUDA_OK(cudaLaunchKernelEx(&cfg, k_gemm_tc<BN, KT, RELU>, mA1, mA2, mB, p));
     SSDNERF_LAUNCH_OK();
     return 0;
 }
@@ -353,7 +355,7 @@ extern "C" int ssdnerf_gemm_f16(const ssdnerf_gemm_args* a, void* stream_) {
     SSDNERF_CUDA_OK(cudaGetDevice(&dev));
     SSDNERF_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     // 3x3 convolution over 128-pixel rows with 128 output channels (the UNet's 128 x 128 level): row-pair kernel with halo reuse
-    if (a->algo != 1 && !kt && a->taps == 9 && !a->tap_offsets && a_stride == 1 && a->d1 == 128 && a->b1 == 128 && a->b2 == 1 && a->b3 == 1 && a->n == 128 && !a->out_f32 && !a->b_batched &&
+    if (a->algo != 1 && !kt && !a->relu && a->taps == 9 && !a->tap_offsets && a_stride == 1 && a->d1 == 128 && a->b1 == 128 && a->b2 == 1 && a->b3 == 1 && a->n == 128 && !a->out_f32 && !a->b_batched &&
         (a->d2 % 2) == 0 && a->alpha == 1.0f && (a->bn == 0 || a->bn == 128) && a->so1 == 128 && a->so2 == 128 * 128 &&
         a->so3 == (long long)a->d2 * 128 * 128 && (!a->qstats || a->stats_hw == 0) && (a->n_rows_b == 0 || a->n_rows_b >= 128))
         return ssdnerf::conv_row2_launch(a, sms, stream);
@@ -362,7 +364,10 @@ extern "C" int ssdnerf_gemm_f16(const ssdnerf_gemm_args* a, void* stream_) {
     if (kt) {
         // the largest tile that divides N; otherwise the one that computes the fewest padding columns (ties: the wider tile)
         const int cand[6] = {256, 160, 80, 48, 40, 16};
-        if (bn) {
+        if (a->relu) {                            // the narrow ReLU instantiation has the 16-column tile only
+            if (bn && bn != 16) return set_error_msg(SSDNERF_ERR_ARG, "gemm (narrow): relu needs bn 0 or 16");
+            bn = 16;
+        } else if (bn) {
             bool ok = false;
             for (int c : cand) ok |= c == bn;
             if (!ok) return set_error_msg(SSDNERF_ERR_ARG, "gemm (narrow): bn must be 16, 40, 48, 80, 160 or 256");
@@ -426,6 +431,12 @@ extern "C" int ssdnerf_gemm_f16(const ssdnerf_gemm_args* a, void* stream_) {
     if (int e = make_map_4d(&mB, a->b, ktot, a->n_rows_b ? a->n_rows_b : a->n, a->bx2 ? a->bx2 : 1, a->bx3 ? a->bx3 : 1, a->b_strides[0],
                             a->b_strides[1], a->b_strides[2], (uint32_t)bn, 1, 1)) return e;
 
+    if (a->relu) {
+        if (kt) return launch_gemm<16, true, true>(mA1, mA2, mB, p, sms, stream);
+        if (bn == 256) return launch_gemm<256, false, true>(mA1, mA2, mB, p, sms, stream);
+        if (bn == 128) return launch_gemm<128, false, true>(mA1, mA2, mB, p, sms, stream);
+        return launch_gemm<64, false, true>(mA1, mA2, mB, p, sms, stream);
+    }
     if (kt) {
         switch (bn) {
             case 256: return launch_gemm<256, true>(mA1, mA2, mB, p, sms, stream);

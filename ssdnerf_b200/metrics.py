@@ -1,4 +1,4 @@
-"""FID / KID over rendered images: the eval-side exchange of the reference (SURVEY.md §8 f3).
+"""SSIM of rendered test views (`ssim`), and FID / KID over rendered images: the eval-side exchange of the reference (SURVEY.md §8 f3).
 
 Surface of lib/core/evaluation/metrics.py:135-215 (`FIDKID(num_images, num_subsets=100, max_subset_size=1000, ...)`, `prepare`, `feed`,
 `summary` -> (fid, fid_mean, fid_cov, kid)) on mmgen's `FID` base [mmgen-memory]: `feed(batch, mode)` extracts features, ALL-GATHERS them
@@ -14,9 +14,24 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
+from . import _lib as N
 from .registry import Registry
 
 METRICS = Registry('metrics')
+
+
+def ssim(pred, target):
+    """per-image SSIM [n] fp32 of channels-last fp32 pred, target [n, h, w, 3] in [0, 1] on the current CUDA device: the reference's
+    `skimage.metrics.structural_similarity(p, t, channel_axis=0, data_range=1)` (lib/core/evaluation/metrics.py:58-71; 7 x 7 uniform
+    window, sample covariance) in one launch (csrc/eval_metrics.cu), with fp64 moments.  h, w >= 7."""
+    N.require_cuda(pred, target)
+    if pred.shape != target.shape or pred.dim() != 4 or pred.shape[-1] != 3:
+        raise ValueError(f'ssim: pred and target must both be [n, h, w, 3], got {tuple(pred.shape)} and {tuple(target.shape)}')
+    pred, target = pred.float().contiguous(), target.float().contiguous()
+    n, h, w, _ = pred.shape
+    out = torch.empty(n, dtype=torch.float32, device=pred.device)
+    N.check(N.lib().ssdnerf_ssim_f32(N.ptr(pred), N.ptr(target), N.c_u32(n), N.c_u32(h), N.c_u32(w), N.ptr(out), N.stream_ptr()))
+    return out
 
 
 def frechet_distance(mean1, cov1, mean2, cov2):

@@ -15,6 +15,7 @@ training) adds the denoiser's weight-gradient pass (unet_train.py, csrc/wgrad.cu
 import functools
 import math
 import os
+import warnings
 from contextlib import contextmanager
 from copy import deepcopy
 
@@ -23,6 +24,7 @@ import torch.nn as nn
 
 from . import _lib as N
 from . import density as D
+from . import metrics as M
 from . import renderer as R
 from .registry import MODELS, MODULES, build_module
 from .scene_cache import SceneCache, restore_optimizer_state
@@ -248,6 +250,10 @@ class BaseNeRF(nn.Module):
         self.test_cfg = test_cfg if test_cfg is not None else dict()
         self.update_extra_interval = update_extra_interval
         self.use_lpips_metric = use_lpips_metric
+        # base_nerf.py:116: a list, so the LPIPS network stays out of the state dict; filled on first use from the default weight files
+        # (ssdnerf_b200/lpips.py), or by the caller with its own `LPIPS(vgg_path, lin_path)`
+        self.lpips = [] if use_lpips_metric else None
+        self._lpips_missing_warned = False
         if init_from_mean:
             self.register_buffer('init_code', torch.zeros(self.code_size))
         else:
@@ -522,9 +528,28 @@ class BaseNeRF(nn.Module):
                            dt_gamma=dt_gamma, want_counts=False)
         return out['rgb'].reshape(num_scenes, num_imgs, h, w, 3), out['depth'].reshape(num_scenes, num_imgs, h, w)
 
+    def _lpips_metric(self):
+        """the LPIPS network of `self.lpips` (an instance, or a list holding one), built from the default weight files on first use;
+        None when the metric is off or the files are missing (warned once)"""
+        from . import lpips as LP
+        if self.lpips is None or isinstance(self.lpips, LP.LPIPS):
+            return self.lpips
+        if len(self.lpips) == 0:
+            if not LP.default_files_exist():
+                if not self._lpips_missing_warned:
+                    vgg, lin = LP.default_paths()
+                    warnings.warn(f'test_lpips is not reported: LPIPS weights not found ({vgg}, {lin or "lpips package not installed"}); '
+                                  'put an ssdnerf_b200.lpips.LPIPS(vgg_path, lin_path) in model.lpips to enable it')
+                    self._lpips_missing_warned = True
+                return None
+            self.lpips.append(LP.LPIPS())
+        return self.lpips[0]
+
     def eval_and_viz(self, data, decoder, code, density_bitfield, viz_dir=None, cfg=dict()):
-        """base_nerf.py:535-673: render, clamp, 8-bit rounding; PSNR against `test_imgs` when present.  SSIM / LPIPS and image files
-        need skimage / lpips / mmcv (not on the hot path, not in this image) and are skipped."""
+        """base_nerf.py:535-673: render, clamp, 8-bit rounding -> `pred_imgs`.  With `test_imgs` in `data` the log holds `test_psnr`
+        (metrics.py:52-55), `test_ssim` (skimage's SSIM, `metrics.ssim`) and, when `use_lpips_metric` is on and LPIPS weights are available
+        (`self.lpips`, see ssdnerf_b200/lpips.py), `test_lpips`: means over all scenes and views.  Without weights `test_lpips` is left out
+        with one warning.  Image files under `viz_dir` (matplotlib / mmcv) are not written."""
         h, w = cfg['img_size']
         image, depth = self.render(decoder, code, density_bitfield, h, w, data['test_intrinsics'], data['test_poses'], cfg=cfg)
         num_scenes, num_imgs = image.shape[:2]
@@ -535,6 +560,13 @@ class BaseNeRF(nn.Module):
             target = data['test_imgs'].permute(0, 1, 4, 2, 3).reshape(num_scenes * num_imgs, 3, h, w)
             mse = (pred_imgs - target).square().flatten(1).mean(dim=1)
             log_vars.update(test_psnr=float((-10 * torch.log10(mse + 1e-6)).mean()))          # eval_psnr (lib/core/evaluation/metrics.py:52-55): eps 1e-6
+            # channels-last views of the same values for the kernels: pred_imgs keeps `image`'s memory order, so this permute copies nothing
+            pred_cl = pred_imgs.permute(0, 2, 3, 1).contiguous()
+            target_cl = data['test_imgs'].reshape(num_scenes * num_imgs, h, w, 3).contiguous()
+            log_vars.update(test_ssim=float(M.ssim(pred_cl, target_cl).mean()))
+            lp = self._lpips_metric()
+            if lp is not None:
+                log_vars.update(test_lpips=float(lp(pred_cl, target_cl).mean()))
         return log_vars, pred_imgs.reshape(num_scenes, num_imgs, 3, h, w)
 
     def mean_ema_update(self, code):

@@ -29,7 +29,7 @@ class GemmArgs(ctypes.Structure):
         ('bn', N.c_u32), ('alpha', N.c_f32), ('bias_n', N.c_void_p), ('residual', N.c_void_p),
         ('out', N.c_void_p), ('out_f32', N.c_u32), ('so1', c_ll), ('so2', c_ll), ('so3', c_ll),
         ('qstats', N.c_void_p), ('stats_hw', N.c_u32), ('algo', N.c_u32),
-        ('tap_offsets', N.c_void_p), ('a_stride', N.c_u32),
+        ('tap_offsets', N.c_void_p), ('a_stride', N.c_u32), ('relu', N.c_u32),
     ]
 
 
@@ -122,9 +122,11 @@ def _conv_boxes_narrow(H, W):
     return bw, bh, 128 // (bw * bh)
 
 
-def conv3x3_f16(x, wp, cout, bias=None, x2=None, residual=None, out=None, out_f32=False, taps=9, bn=0, qstats=None, algo=0, narrow=False):
+def conv3x3_f16(x, wp, cout, bias=None, x2=None, residual=None, out=None, out_f32=False, taps=9, bn=0, qstats=None, algo=0, narrow=False,
+                relu=False):
     """3x3 (taps=9, pad 1, stride 1) or 1x1 (taps=1) convolution over NHWC fp16 x [B,H,W,C1] (+ x2 [B,H,W,C2] concatenated
-    along channels).  wp: packed weight [taps][Cout_pad][C1+C2].  narrow: C1 / C2 multiples of 8 (narrow-channel family)."""
+    along channels).  wp: packed weight [taps][Cout_pad][C1+C2].  narrow: C1 / C2 multiples of 8 (narrow-channel family).
+    relu: max(0, .) in the epilogue (generic tile kernel; narrow: 16-column N tiles)."""
     N.require_cuda(x, wp)
     B, H, W, C1 = x.shape
     C2 = x2.shape[-1] if x2 is not None else 0
@@ -156,6 +158,7 @@ def conv3x3_f16(x, wp, cout, bias=None, x2=None, residual=None, out=None, out_f3
     g.so1, g.so2, g.so3 = co, W * co, H * W * co
     if qstats is not None:
         g.qstats, g.stats_hw = qstats.data_ptr(), 0
+    g.relu = int(relu)
     _launch(g)
     return out
 
