@@ -396,6 +396,30 @@ SSDNERF_API uint32_t ssdnerf_lpips_tap_partials(uint32_t m, uint32_t h, uint32_t
 SSDNERF_API int ssdnerf_lpips_tap_f16(const void* feat, uint32_t m, uint32_t h, uint32_t w, uint32_t c, const float* lin, float* partial,
                                      void* pooled, float* out, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * 6. Mesh extraction: marching cubes over a density lattice (csrc/mesh.cu).
+ *    replaces: mcubes.marching_cubes(u, threshold) in lib/core/utils/nerf_utils.py:84-112, called by
+ *              lib/models/autodecoders/base_nerf.py:172-182 (save_mesh).
+ *    u fp32 [nx][ny][nz] (C order, indexed [x][y][z]).  A lattice point is low when u <= threshold (fp64 compare); every crossed
+ *    lattice edge carries one vertex, in lattice-index units, its axis coordinate (x2 - x1) * (thr - f1) / (f2 - f1) + x1 in fp64
+ *    from the edge's lower end.  Vertices are ordered by edge id 3 * ((x * ny + y) * nz + z) + axis, triangles by the cube's
+ *    lower-corner linear index, then by the generated case table (ssdnerf_mc_case_table), whose triangle normals
+ *    (v1 - v0) x (v2 - v0) point to the low side and whose ambiguous faces are resolved alike by both cubes (watertight).
+ *    Two passes: ssdnerf_mc_count, one host read of counts[2] = {vertices, triangles}, ssdnerf_mc_emit with the same u, threshold
+ *    and workspace.  A dimension below 2 gives an empty mesh; 3 * nx * ny * nz >= 2^32 is SSDNERF_ERR_ARG.  Deterministic.
+ * ---------------------------------------------------------------------------------------------- */
+/* bytes of workspace (8-byte aligned) for ssdnerf_mc_count / ssdnerf_mc_emit: about 1.8 per lattice point; 0 for an empty mesh */
+SSDNERF_API size_t ssdnerf_mc_workspace_bytes(uint32_t nx, uint32_t ny, uint32_t nz);
+SSDNERF_API int ssdnerf_mc_count(const float* u, uint32_t nx, uint32_t ny, uint32_t nz, double threshold, void* workspace,
+                                 unsigned long long* counts /* [2] */, void* stream);
+/* vertices fp64 [V][3], triangles int64 [T][3] (sizes from counts; nothing to emit when both are 0) */
+SSDNERF_API int ssdnerf_mc_emit(const float* u, uint32_t nx, uint32_t ny, uint32_t nz, double threshold, const void* workspace,
+                                double* vertices, long long* triangles, void* stream);
+/* host copy of the case table: tri_count_host [256], tri_host [256][10][3] cube-edge numbers (zero past the count).  Corner i of a
+ * cube is at (i & 1, (i >> 1) & 1, (i >> 2) & 1) in (x, y, z) and low corners set bit i of the case; cube edge 4 a + k runs along
+ * axis a from the corner whose other two axes b < c are k & 1 and k >> 1 */
+SSDNERF_API int ssdnerf_mc_case_table(uint8_t* tri_count_host, uint8_t* tri_host);
+
 #ifdef __cplusplus
 }
 #endif

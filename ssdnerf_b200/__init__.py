@@ -4,12 +4,13 @@
     density             : occupancy-grid builder                   (csrc/density.cu)
     unet / diffusion    : DDIM loop over triplane latents          (csrc/gemm_tc.cu, csrc/unet_glue.cu)
     raymarching / shencoder / activation : one-to-one mirrors of the reference's lib.ops (csrc/legacy_ops.cu)
+    mesh                : marching cubes + binary STL of save_mesh  (csrc/mesh.cu)
 
 Everything computes through libssdnerf_b200.so (C ABI: include/ssdnerf_b200.h); there is no CPU or PyTorch fallback.
 """
 from .registry import MODELS, MODULES, build_model, build_module  # noqa: F401
 from .config import Config  # noqa: F401
-from . import activation, decoders, density, diffusion, nerf, raymarching, renderer, scene_cache, shencoder, unet  # noqa: F401
+from . import activation, decoders, density, diffusion, mesh, nerf, raymarching, renderer, scene_cache, shencoder, unet  # noqa: F401
 from .decoders import TriPlaneDecoder  # noqa: F401
 from .diffusion import GaussianDiffusion  # noqa: F401
 from .nerf import DiffusionNeRF, MultiSceneNeRF  # noqa: F401

@@ -14,6 +14,7 @@ _lib = None
 c_void_p = ctypes.c_void_p
 c_u32 = ctypes.c_uint32
 c_f32 = ctypes.c_float
+c_double = ctypes.c_double
 c_int = ctypes.c_int
 c_size_t = ctypes.c_size_t
 c_longlong = ctypes.c_longlong
@@ -71,6 +72,12 @@ def lib():
                      'ssdnerf_density_workspace_bytes', 'ssdnerf_unet_workspace_bytes'):
             if hasattr(L, name):
                 getattr(L, name).restype = c_size_t
+        # mesh extraction (header section 6)
+        L.ssdnerf_mc_workspace_bytes.argtypes = [c_u32, c_u32, c_u32]
+        L.ssdnerf_mc_workspace_bytes.restype = c_size_t
+        L.ssdnerf_mc_count.argtypes = [c_void_p, c_u32, c_u32, c_u32, c_double, c_void_p, c_void_p, c_void_p]
+        L.ssdnerf_mc_emit.argtypes = [c_void_p, c_u32, c_u32, c_u32, c_double, c_void_p, c_void_p, c_void_p, c_void_p]
+        L.ssdnerf_mc_case_table.argtypes = [c_void_p, c_void_p]
         _lib = L
     return _lib
 

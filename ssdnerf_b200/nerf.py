@@ -24,6 +24,7 @@ import torch.nn as nn
 
 from . import _lib as N
 from . import density as D
+from . import mesh as MC
 from . import metrics as M
 from . import renderer as R
 from .registry import MODELS, MODULES, build_module
@@ -178,14 +179,12 @@ def extract_fields(decoder, code_single, resolution=256, margin=0.1):
 
 
 def extract_geometry(decoder, code_single, resolution=256, threshold=10):
-    """nerf_utils.py:84-112: marching cubes (PyMCubes, as in the reference) over `extract_fields`"""
-    try:
-        import mcubes
-    except ImportError as e:
-        raise ImportError('extract_geometry needs PyMCubes (`mcubes`), like the reference') from e
+    """nerf_utils.py:84-112: marching cubes on the device (`mesh.marching_cubes`, PyMCubes' contract) over `extract_fields`, mapped to
+    world coordinates by the reference's formula.  Returns numpy float64 vertices [V, 3] and int64 triangles [T, 3]."""
     with torch.no_grad():
-        u = extract_fields(decoder, code_single, resolution).cpu().numpy()
-    vertices, triangles = mcubes.marching_cubes(u, threshold)
+        u = extract_fields(decoder, code_single, resolution)
+    vertices, triangles = MC.marching_cubes(u, threshold)
+    vertices, triangles = vertices.cpu().numpy(), triangles.cpu().numpy()
     lo = (decoder.aabb[:3] - 0.1).cpu().numpy()
     hi = (decoder.aabb[3:] + 0.1).cpu().numpy()
     return vertices / (resolution - 1.0) * (hi - lo)[None, :] + lo[None, :], triangles
@@ -305,16 +304,12 @@ class BaseNeRF(nn.Module):
 
     @staticmethod
     def save_mesh(save_dir, decoder, code, scene_name, mesh_resolution, mesh_threshold):
-        """base_nerf.py:172-182: density field on the device (`extract_fields`), surface by PyMCubes, file by trimesh -- the two
-        packages the reference uses for this; neither is part of this image, so the call fails loudly when they are missing."""
-        try:
-            import trimesh
-        except ImportError as e:
-            raise ImportError('save_mesh needs `trimesh` (and `mcubes`), like the reference (requirements.txt)') from e
+        """base_nerf.py:172-182: one binary `<scene_name>.stl` per scene -- density lattice and marching cubes on the device
+        (`extract_geometry`), file by `mesh.write_stl`"""
         os.makedirs(save_dir, exist_ok=True)
         for code_single, name in zip(code, scene_name):
             vertices, triangles = extract_geometry(decoder, code_single, mesh_resolution, mesh_threshold)
-            trimesh.Trimesh(vertices, triangles, process=False).export(os.path.join(save_dir, name) + '.stl')
+            MC.write_stl(os.path.join(save_dir, name) + '.stl', vertices, triangles)
 
     def get_init_code_(self, num_scenes, device=None):
         code_ = torch.empty(self.code_size if num_scenes is None else (num_scenes, *self.code_size), device=device, requires_grad=True,
