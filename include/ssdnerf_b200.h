@@ -420,6 +420,33 @@ SSDNERF_API int ssdnerf_mc_emit(const float* u, uint32_t nx, uint32_t ny, uint32
  * axis a from the corner whose other two axes b < c are k & 1 and k >> 1 */
 SSDNERF_API int ssdnerf_mc_case_table(uint8_t* tri_count_host, uint8_t* tri_host);
 
+/* ------------------------------------------------------------------------------------------------
+ * 7. Inception-v3 features of FID / KID (csrc/inception.cu), NHWC fp16 activations.
+ *    replaces: the StyleGAN Inception TorchScript (`inception_args=dict(type='StyleGAN', ...)`) that mmgen's FID and the
+ *              reference's FIDKID (lib/core/evaluation/metrics.py) run on `feed`'s [-1, 1] images.
+ *    A tensor "in a channel slice" has pixel p, channel k at base[p * stride + k]: the caller offsets the pointer to the slice.
+ *    Every output element comes from one thread in a fixed order (no atomics): bit-identical run to run, independent of n.
+ * ---------------------------------------------------------------------------------------------- */
+/* x fp32 [n][3][h][w] in [-1, 1] -> u = uint8(clamp(x * 127.5 + 128, 0, 255)) (multiply and add rounded separately, truncating
+ * cast), resized to 299 x 299 when (h, w) != (299, 299) by sampling source coordinate o * in / 299 bilinearly, clamped to the last
+ * pixel, then (u - 128) / 128 -> out fp16 [n][299][299][16] (channels 3..15 zero).  u8 != NULL also receives u, [n][3][h][w]. */
+SSDNERF_API int ssdnerf_incep_prep_f16(const float* x, uint32_t n, uint32_t h, uint32_t w, void* out, uint8_t* u8, void* stream);
+/* y = [relu](conv(x, weight) + bias), x [n][h][w] pixels of `cin` channels at pixel stride x_stride, weight fp16 [cout][kh][kw][cin],
+ * bias fp32 [cout] (may be NULL), y [n][oh][ow] pixels of `cout` channels at pixel stride y_stride, oh = (h + 2 pad_h - kh) / stride + 1
+ * (likewise ow).  cin % 16 == 0, cout % 8 == 0, strides multiples of 8, stride 1 or 2, kh * kw <= 64, pad < kernel extent.
+ * Implicit GEMM on wgmma (fp32 accumulation, one fp16 rounding at the store). */
+SSDNERF_API int ssdnerf_incep_conv_f16(const void* x, uint32_t n, uint32_t h, uint32_t w, uint32_t cin, uint32_t x_stride, const void* weight,
+                                       const float* bias, uint32_t cout, uint32_t kh, uint32_t kw, uint32_t stride, uint32_t pad_h,
+                                       uint32_t pad_w, int relu, void* y, uint32_t y_stride, void* stream);
+#define SSDNERF_POOL_MAX_S2 0   /* 3 x 3 max, stride 2, no padding: oh = (h - 3) / 2 + 1 */
+#define SSDNERF_POOL_AVG_S1 1   /* 3 x 3 average, stride 1, pad 1, padding excluded from the count */
+#define SSDNERF_POOL_MAX_S1 2   /* 3 x 3 max, stride 1, pad 1 */
+/* 3 x 3 pool of x ([n][h][w] pixels of c channels at stride x_stride) into y (pixel stride y_stride); c and strides multiples of 8 */
+SSDNERF_API int ssdnerf_incep_pool_f16(const void* x, uint32_t n, uint32_t h, uint32_t w, uint32_t c, uint32_t x_stride, int mode, void* y,
+                                       uint32_t y_stride, void* stream);
+/* out fp32 [n][c] = mean over the hw pixels of x fp16 [n][hw][c], summed in pixel order */
+SSDNERF_API int ssdnerf_incep_mean_f16(const void* x, uint32_t n, uint32_t hw, uint32_t c, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -6,8 +6,10 @@ across ranks (lib/apis/test.py:41-53 is the caller; this is the only collective 
 
 What differs: features stay on the device, the statistics are computed there in float64 (mean / covariance as one GEMM, the matrix square
 root of the Frechet distance from a symmetric eigendecomposition, KID as batched GEMMs over all subsets at once), and the feature extractor
-is a plug-in callable -- the StyleGAN Inception-v3 TorchScript (`inception_args`) is an external asset that is not available offline, so
-`feature_fn` must be supplied (any [n,3,h,w] float in [-1, 1] -> [n, D] tensor)."""
+is either a plug-in callable `feature_fn` (any [n,3,h,w] float in [-1, 1] -> [n, D] tensor) or, by default, the package's native
+Inception-v3 (ssdnerf_b200.inception) loaded at the first `feed` from the StyleGAN TorchScript named by
+`inception_args=dict(type='StyleGAN', inception_path=...)`, an external asset that is never downloaded."""
+import os
 import pickle
 
 import numpy as np
@@ -78,6 +80,7 @@ class FIDKID:
                  bgr2rgb=False, image_shape=None):
         self.num_images, self.num_subsets, self.max_subset_size = num_images, num_subsets, max_subset_size
         self.feature_fn, self.inception_pkl, self.bgr2rgb = feature_fn, inception_pkl, bgr2rgb
+        self.inception_args = dict(inception_args) if inception_args else None
         self.real_feats, self.fake_feats = [], []
         self.num_real_feeded = self.num_fake_feeded = 0
         self.real_mean = self.real_cov = self.real_feats_all = None
@@ -100,6 +103,21 @@ class FIDKID:
             self.real_feats_all = torch.as_tensor(ref['feats_np'])
             self.num_real_feeded = self.num_images
 
+    def _native_extractor(self):
+        """the package's Inception-v3 (ssdnerf_b200.inception) with the weights of `inception_args['inception_path']`, loaded on first
+        use; the file is never downloaded"""
+        args = self.inception_args
+        if not args:
+            raise RuntimeError('FIDKID needs `feature_fn` or `inception_args=dict(type=\'StyleGAN\', inception_path=...)`')
+        if args.get('type') != 'StyleGAN':
+            raise NotImplementedError(f'FIDKID: inception_args type {args.get("type")!r} is not supported (only \'StyleGAN\')')
+        path = args.get('inception_path')
+        if not path or not os.path.isfile(path):
+            raise RuntimeError(f'FIDKID: the Inception-v3 TorchScript {path!r} was not found (it is an external asset and is never '
+                               'downloaded; pass `feature_fn` or place the file there)')
+        from .inception import InceptionV3
+        return InceptionV3.load(path)
+
     def feed(self, batch, mode):
         """batch [n,3,h,w] in [-1, 1] -> features -> all-gather over the default process group -> keep what is still needed.
         Returns the number of rows kept (mmgen FID.feed contract [mmgen-memory])."""
@@ -108,7 +126,7 @@ class FIDKID:
         if need <= 0:
             return 0
         if self.feature_fn is None:
-            raise RuntimeError('FIDKID needs `feature_fn` (the Inception-v3 TorchScript of the reference is an external asset)')
+            self.feature_fn = self._native_extractor()
         if self.bgr2rgb:
             batch = batch[:, [2, 1, 0]]
         with torch.no_grad():
