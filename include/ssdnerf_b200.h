@@ -231,8 +231,8 @@ SSDNERF_API int ssdnerf_density_pack(const void* density_grid, int grid_is_half,
  *    memory-bound glue kernels).  Activations are NHWC fp16; accumulation is fp32.
  *    replaces: cuDNN/cuBLAS calls under lib/models/architecture/ddpm/denoising.py:191-216 and
  *              modules.py:28-48 (+ mmgen 0.7.2 DenoisingResBlock / NormWithEmbedding / QKVAttention /
- *              DenoisingDownsample / DenoisingUpsample forwards), and the DDIM algebra of
- *              lib/models/diffusions/gaussian_diffusion.py:180-240,264-293.
+ *              DenoisingDownsample / DenoisingUpsample forwards), and the DDIM / DDPM algebra of
+ *              lib/models/diffusions/gaussian_diffusion.py:156-164,180-240,264-293,333-386.
  * ---------------------------------------------------------------------------------------------- */
 typedef struct ssdnerf_gemm_args {
     /* D[m, n] = alpha * sum_{tap,k} A_tap[m, k] * B[tap][n, k] + bias_n[n] + residual[m, n]
@@ -297,6 +297,15 @@ SSDNERF_API int ssdnerf_transpose_v(const void* qkv, uint32_t B, uint32_t T, uin
 SSDNERF_API int ssdnerf_ddim_update(float* x_t, const float* v, uint32_t B, uint32_t C, uint32_t H, uint32_t W, uint32_t Cv,
                                     const float* coef, const int* step_ptr, int clip, float clip_lo, float clip_hi, float* x0_out,
                                     void* next_in, uint32_t Cpad, void* stream);
+/* One DDPM step of the V-parameterisation (gaussian_diffusion.py:156-164,333-386, csrc/ddpm.cu), x_t fp32 [B,C,H,W] updated in place:
+ *   x0 = clamp(c0*x_t - c1*v);  x_prev = (c2*x0 + c3*x_t) + c4*z,  coef[step] = {c0,c1,c2,c3,c4} (c4 = (t != 0) sqrt(var_t)),
+ * every product and sum rounded on its own.  z ~ N(0, 1) is generated in the kernel: Philox4x32-10 with key *seed_ptr and counter
+ * {index lo, index hi, step, 0} for the NCHW element index of x_t, Box-Muller r = sqrt(-2 log u0) cos(2 pi u1) with
+ * u0 = ((w0 >> 8) | 1) 2^-24 and u1 = (w1 >> 8) 2^-24 -- a value depends only on (seed, step, index).  The row {0,0,0,0,1} writes z.
+ * v fp32 NHWC [B,H,W,Cv], Cv >= C; step index read from *step_ptr; optionally writes the next UNet input (fp16 NHWC, Cpad). */
+SSDNERF_API int ssdnerf_ddpm_update(float* x_t, const float* v, uint32_t B, uint32_t C, uint32_t H, uint32_t W, uint32_t Cv,
+                                    const float* coef, const int* step_ptr, const unsigned long long* seed_ptr, int clip, float clip_lo,
+                                    float clip_hi, void* next_in, uint32_t Cpad, void* stream);
 /* device-side step bookkeeping of the graph-replayed DDIM loop: *step_ptr = value (set) or += value; and
  * dst[c][:] = table[*step_ptr][:] for c < copies (selects the per-step time-embedding projections) */
 SSDNERF_API int ssdnerf_step_counter(int* step_ptr, int value, int set, void* stream);

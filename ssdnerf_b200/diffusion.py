@@ -1,12 +1,13 @@
-"""`GaussianDiffusion` -- DDIM sampling over triplane latents, driven from one CUDA stream.
+"""`GaussianDiffusion` -- DDIM and DDPM sampling over triplane latents, driven from one CUDA stream.
 
-Plugin surface of lib/models/diffusions/gaussian_diffusion.py:14-464 (constructor kwargs, `forward`, `ddim_sample`,
+Plugin surface of lib/models/diffusions/gaussian_diffusion.py:14-464 (constructor kwargs, `forward`, `ddim_sample`, `ddpm_sample`,
 `sample_from_noise`, `pred_x_0`, schedule attributes, `test_cfg` read at call time).  The sampler differs in HOW it
 runs: the reference re-uploads a 1000-entry table and syncs device->host several times per step
 (gaussian_diffusion.py:190-191,275-279,302-304); here the timestep list and all coefficients are computed once on the
 host (float64, like the reference's NumPy tables), the per-step time-embedding projections are precomputed for every
-step, and ONE captured CUDA graph (UNet forward + fused V->x0->eps->x_prev update, device-side step counter) is
-replayed `num_timesteps` times.
+step, and ONE captured CUDA graph (UNet forward + fused update, device-side step counter) is replayed `num_timesteps`
+times.  The fused update is V->x0->eps->x_prev for DDIM and V->x0->posterior mean + sigma * noise for DDPM, whose noise
+the kernel generates from a per-call seed in device memory.
 """
 import math
 import os
@@ -291,6 +292,34 @@ class GaussianDiffusion(nn.Module):
             x_prev = x_prev + eta * float(np.sqrt(tilde_beta_t)) * noise
         return x_prev, x_0_pred
 
+    def _table_f32(self, x, table, t):
+        """mmgen's var_to_tensor: the float64 table entry at t rounded to float32, shaped to broadcast over x"""
+        return torch.from_numpy(np.asarray(table))[torch.as_tensor(t).cpu()].float().to(x.device).reshape(-1, 1, 1, 1)
+
+    def q_posterior_mean(self, x_0, x_t, t):
+        """gaussian_diffusion.py:156-164"""
+        return self._table_f32(x_0, self.tilde_mu_t_coef1, t) * x_0 + self._table_f32(x_0, self.tilde_mu_t_coef2, t) * x_t
+
+    def _ddpm_var_table(self):
+        """gaussian_diffusion.py:343-349: FIXED_LARGE indexes [tilde_beta_1, betas...] at t, i.e. betas[t - 1] for t >= 1"""
+        mode = self.denoising_var_mode.upper()
+        if mode == 'FIXED_LARGE':
+            return np.append(self.tilde_betas_t[1], self.betas)
+        if mode == 'FIXED_SMALL':
+            return self.tilde_betas_t
+        raise AttributeError(f'Unknown denoising var output type [{self.denoising_var_mode}].')
+
+    @torch.no_grad()
+    def p_sample_ddpm(self, x_t, t, noise=None, cfg=dict(), grad_guide_fn=None, **kwargs):
+        """gaussian_diffusion.py:333-365: posterior mean of the predicted x_0, plus sqrt(var_t) * noise unless t == 0"""
+        var = self._table_f32(x_t, self._ddpm_var_table(), t)
+        x_0_pred, _ = self.pred_x_0(x_t, torch.as_tensor(t, device=x_t.device), grad_guide_fn=grad_guide_fn, cfg=cfg, **kwargs)
+        mean = self.q_posterior_mean(x_0_pred, x_t, t)
+        if noise is None:
+            noise = torch.randn_like(x_t)
+        nonzero_mask = (torch.as_tensor(t) != 0).float().reshape(-1, 1, 1, 1).to(x_t.device)
+        return mean + nonzero_mask * torch.sqrt(var) * noise, x_0_pred
+
     @torch.no_grad()
     def _ddim_sample_stepwise(self, noise, concat_cond=None, save_intermediates=False, grad_guide_fn=None, langevin_noises=None,
                               show_pbar=False, **kwargs):
@@ -332,7 +361,7 @@ class GaussianDiffusion(nn.Module):
                          np.sqrt(1 - ab_prev - self.tilde_betas_t[t] * eta ** 2)])
         return torch.tensor(np.asarray(rows, np.float64), dtype=torch.float32)
 
-    # ------------------------------------------------------------------ the loop
+    # ------------------------------------------------------------------ the loops
     @torch.no_grad()
     def ddim_sample(self, noise, show_pbar=False, concat_cond=None, save_intermediates=False, use_graph=True, **kwargs):
         """gaussian_diffusion.py:295-331.  Unguided eta=0 V-parameterisation (every unconditional config) = captured graph;
@@ -345,21 +374,86 @@ class GaussianDiffusion(nn.Module):
         if concat_cond is not None:
             raise NotImplementedError('concat_cond (image-conditioned denoiser) is not used by the shipped configs')
         N.require_cuda(noise)
+        B, C, H, W = noise.shape
+        # Lanes (optional): the batch can be split into independent sub-batches, each with its own engine, captured step and CUDA stream.
+        # The persistent GEMM kernels own all SMs, so lanes serialise and only add launches; the default stays 1.
+        n_lanes = int(os.environ.get('SSDNERF_DDIM_STREAMS', cfg.get('ddim_streams', 1)))
+        if n_lanes < 1 or B % n_lanes or not use_graph:
+            n_lanes = 1
+        st = self._sampler_state('ddim', noise, use_graph, n_lanes, lambda ts: self.ddim_coefficients(ts, eta))
+        L = N.lib()
+
+        def update(ln, v, s):
+            eng = ln['eng']
+            N.check(L.ssdnerf_ddim_update(N.ptr(ln['x_t']), N.ptr(v), N.c_u32(ln['hi'] - ln['lo']), N.c_u32(C), N.c_u32(H), N.c_u32(W),
+                                          N.c_u32(v.shape[-1]), N.ptr(st['coef']), N.ptr(ln['step_ptr']), N.c_int(int(st['clip'])),
+                                          N.c_f32(st['clip_range'][0]), N.c_f32(st['clip_range'][1]), None, N.ptr(eng.x_in), N.c_u32(eng.CPAD_IN), s))
+        return self._run_sampler(st, noise, update, use_graph)
+
+    @torch.no_grad()
+    def _ddpm_sample_stepwise(self, noise, grad_guide_fn=None, ddpm_noises=None, **kwargs):
+        """gaussian_diffusion.py:367-386 step by step (host timesteps): guidance, EPS / START_X denoisers and injected noise.
+        `ddpm_noises`: optional iterator of the tensors the steps add (parity tests; default torch.randn, as the reference)."""
+        cfg = self.test_cfg
+        x_t = noise.detach().float()
+        for t in self.ddim_timesteps(cfg.get('num_timesteps', self.num_timesteps)).tolist():
+            x_t, _ = self.p_sample_ddpm(x_t, t, noise=next(ddpm_noises) if ddpm_noises is not None else None, cfg=cfg,
+                                        grad_guide_fn=grad_guide_fn, **kwargs)
+        return x_t
+
+    def ddpm_coefficients(self, timesteps):
+        """float64 host tables -> fp32 rows {sqrt(ab_t), sqrt(1-ab_t), coef1_t, coef2_t, (t != 0) sqrt(var_t)} (:156-164,333-365):
+        each table entry rounded to float32 (var_to_tensor), the square root of the variance taken in float32 (torch.sqrt)"""
+        var = self._ddpm_var_table()
+        rows = []
+        for t in (int(t) for t in timesteps):
+            rows.append([np.float32(self.sqrt_alphas_bar[t]), np.float32(self.sqrt_one_minus_alphas_bar[t]), np.float32(self.tilde_mu_t_coef1[t]),
+                         np.float32(self.tilde_mu_t_coef2[t]), np.sqrt(np.float32(var[t])) if t != 0 else np.float32(0)])
+        return torch.from_numpy(np.asarray(rows, np.float32))
+
+    @torch.no_grad()
+    def ddpm_sample(self, noise, show_pbar=False, concat_cond=None, use_graph=True, ddpm_noises=None, **kwargs):
+        """gaussian_diffusion.py:367-386: the posterior step at each of the strided timesteps of `ddim_timesteps`.  Unguided V-parameterisation
+        = captured graph (UNet forward + ssdnerf_ddpm_update, whose noise is generated in the kernel from a seed drawn per call with
+        `torch.empty(1, dtype=torch.int64).random_()`, so `torch.manual_seed` makes a call repeatable); guidance, EPS / START_X and
+        injected `ddpm_noises` = the step-wise loop."""
+        if 'save_intermediates' in kwargs:
+            raise TypeError('ddpm_sample keeps no intermediates: save_intermediates is a ddim_sample option')
+        if concat_cond is not None:
+            raise NotImplementedError('concat_cond (image-conditioned denoiser) is not used by the shipped configs')
+        self._ddpm_var_table()                # an unknown denoising_var_mode raises before any work, as in p_sample_ddpm
+        if kwargs.get('grad_guide_fn') is not None or ddpm_noises is not None or self.denoising_mean_mode.upper() != 'V':
+            return self._ddpm_sample_stepwise(noise, ddpm_noises=ddpm_noises, **kwargs)
+        N.require_cuda(noise)
+        B, C, H, W = noise.shape
+        st = self._sampler_state(('ddpm', self.denoising_var_mode.upper()), noise, use_graph, 1, self.ddpm_coefficients)
+        if 'seed' not in st:
+            st['seed'] = torch.empty(1, dtype=torch.int64, device=noise.device)
+        st['seed'].copy_(torch.empty(1, dtype=torch.int64).random_())
+        L = N.lib()
+
+        def update(ln, v, s):
+            eng = ln['eng']
+            N.check(L.ssdnerf_ddpm_update(N.ptr(ln['x_t']), N.ptr(v), N.c_u32(B), N.c_u32(C), N.c_u32(H), N.c_u32(W), N.c_u32(v.shape[-1]),
+                                          N.ptr(st['coef']), N.ptr(ln['step_ptr']), N.ptr(st['seed']), N.c_int(int(st['clip'])),
+                                          N.c_f32(st['clip_range'][0]), N.c_f32(st['clip_range'][1]), N.ptr(eng.x_in), N.c_u32(eng.CPAD_IN), s))
+        return self._run_sampler(st, noise, update, use_graph)
+
+    def _sampler_state(self, kind, noise, use_graph, n_lanes, coef_fn):
+        """The state of a device-side sampling loop: per lane an engine, an x_t buffer and a device step counter; the fp32 coefficient
+        rows `coef_fn(timesteps)` and every step's time-embedding projections (host precompute, no x dependence).  One entry per
+        (sampler kind, denoiser weights, device, batch shape, sampler settings); a ragged last batch alternates between two entries instead of
+        re-capturing.  Stale entries (changed weights) and anything beyond 4 entries are dropped, oldest first."""
+        cfg = self.test_cfg
         num_steps = cfg.get('num_timesteps', self.num_timesteps)
         clip = bool(cfg.get('clip_denoised', True))
         clip_range = tuple(float(c) for c in cfg.get('clip_range', [-1, 1]))
         dev = noise.device
         B, C, H, W = noise.shape
         unet = self.denoising
-        # Lanes (optional): the batch can be split into independent sub-batches, each with its own engine, captured step and CUDA stream.
-        # The persistent GEMM kernels own all SMs, so lanes serialise and only add launches; the default stays 1.
-        n_lanes = int(os.environ.get('SSDNERF_DDIM_STREAMS', cfg.get('ddim_streams', 1)))
-        if n_lanes < 1 or B % n_lanes or not use_graph:
-            n_lanes = 1
         Bl = B // n_lanes
-        key = (id(unet), tuple(p._version for p in unet.parameters()), str(dev), B, C, H, W, num_steps, clip, clip_range, bool(use_graph), n_lanes)
-        # one captured state per (device, batch shape, sampler settings); a ragged last batch alternates between two entries instead of
-        # re-capturing.  Stale entries (changed weights) and anything beyond 4 entries are dropped, oldest first.
+        key = (id(unet), tuple(p._version for p in unet.parameters()), str(dev), B, C, H, W, num_steps, clip, clip_range, bool(use_graph), n_lanes,
+               kind)
         for k in [k for k in self._graphs if k[0] == id(unet) and k[1] != key[1]]:
             del self._graphs[k]
         st = self._graphs.get(key)
@@ -373,24 +467,26 @@ class GaussianDiffusion(nn.Module):
                                   stream=torch.cuda.Stream(device=dev) if n_lanes > 1 else None,
                                   x_t=torch.empty(Bl, C, H, W, dtype=torch.float32, device=dev),
                                   step_ptr=torch.zeros(1, dtype=torch.int32, device=dev)))
-            st = dict(key=key, S=len(ts), lanes=lanes,
-                      # host-side precompute (no x dependence): coefficient rows + every step's scale/shift projections
-                      coef=self.ddim_coefficients(ts, eta).to(dev),
+            st = dict(key=key, S=len(ts), lanes=lanes, clip=clip, clip_range=clip_range, coef=coef_fn(ts).to(dev),
                       ss_table=lanes[0]['eng'].scale_shift_rows(unet.embedding(ts.to(dev))).contiguous())          # [S, ss_total]
             while len(self._graphs) >= 4:
                 del self._graphs[next(iter(self._graphs))]
             self._graphs[key] = st
-        coef, ss_table, S, lanes = st['coef'], st['ss_table'], st['S'], st['lanes']
+        return st
+
+    def _run_sampler(self, st, noise, update, use_graph):
+        """S steps of [select the step's embedding rows, UNet forward, `update(lane, v, stream)`, advance the step counter]: S replays of
+        each lane's captured step on its stream, or (`use_graph=False`) the same launches uncaptured"""
+        ss_table, S, lanes = st['ss_table'], st['S'], st['lanes']
+        dev = noise.device
+        n_lanes = len(lanes)
         L = N.lib()
 
         def one_step(ln):
-            eng, x_t, step_ptr = ln['eng'], ln['x_t'], ln['step_ptr']
+            eng, step_ptr = ln['eng'], ln['step_ptr']
             s = N.stream_ptr()
-            N.check(L.ssdnerf_select_row(N.ptr(ss_table), N.c_u32(eng.ss_total), N.ptr(step_ptr), N.ptr(eng.ss_cur), N.c_u32(Bl), s))
-            v = eng.forward_nhwc()
-            N.check(L.ssdnerf_ddim_update(N.ptr(x_t), N.ptr(v), N.c_u32(Bl), N.c_u32(C), N.c_u32(H), N.c_u32(W), N.c_u32(v.shape[-1]),
-                                          N.ptr(coef), N.ptr(step_ptr), N.c_int(int(clip)), N.c_f32(clip_range[0]), N.c_f32(clip_range[1]),
-                                          None, N.ptr(eng.x_in), N.c_u32(eng.CPAD_IN), s))
+            N.check(L.ssdnerf_select_row(N.ptr(ss_table), N.c_u32(eng.ss_total), N.ptr(step_ptr), N.ptr(eng.ss_cur), N.c_u32(ln['hi'] - ln['lo']), s))
+            update(ln, eng.forward_nhwc(), s)
             N.check(L.ssdnerf_step_counter(N.ptr(step_ptr), N.c_int(1), N.c_int(0), s))
 
         def reset(ln):
