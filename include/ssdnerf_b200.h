@@ -456,6 +456,35 @@ SSDNERF_API int ssdnerf_incep_pool_f16(const void* x, uint32_t n, uint32_t h, ui
 /* out fp32 [n][c] = mean over the hw pixels of x fp16 [n][hw][c], summed in pixel order */
 SSDNERF_API int ssdnerf_incep_mean_f16(const void* x, uint32_t n, uint32_t hw, uint32_t c, float* out, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * 8. PNG files of evaluation images (csrc/png.cu): 8-bit RGBA (colour type 6), non-interlaced, one IDAT, as plt.imsave writes.
+ *    replaces: plt.imsave in lib/models/autodecoders/base_nerf.py:574-608 (eval_and_viz) and
+ *              lib/models/decoders/triplane_decoder.py:186-194 (visualize).
+ *    The contract is the decoded pixels; the compressed bytes are this encoder's own (adaptive filters by libpng's
+ *    minimum-sum heuristic, dynamic-Huffman deflate in segments of whole rows).  A file's bytes depend only on its pixels.
+ *    Output: file i is out[offsets[i] : offsets[i + 1]], offsets uint64 [n + 1] on the device (offsets[n] = total).
+ *    n, h, w >= 1 and a row of 4 w + 1 bytes at most SSDNERF_PNG_SEGMENT_BYTES, else SSDNERF_ERR_ARG; so are a workspace or
+ *    output smaller than the queries below.
+ * ---------------------------------------------------------------------------------------------- */
+#define SSDNERF_PNG_SEGMENT_BYTES 16384
+/* bytes of workspace (256-byte aligned) for n images of h x w output pixels; 0 for invalid sizes */
+SSDNERF_API size_t ssdnerf_png_workspace_bytes(uint32_t n, uint32_t h, uint32_t w);
+/* the largest total the n files can take: n * (63 + h * (4 w + 1) + 5 * segments per image); 0 for invalid sizes */
+SSDNERF_API size_t ssdnerf_png_output_bound(uint32_t n, uint32_t h, uint32_t w);
+/* view images of eval_and_viz: pred, real fp32 [n][h][w_view][3] channels-last.  Prediction bytes are
+ * round(float32(round(clamp(x, 0, 1) * 255) / 255) * 255) (both roundings half to even); real bytes (t * 255) truncated.  With real,
+ * the file is 2 w_view wide, real left of pred; without, w_view.  Alpha 255.  Size queries take the file width. */
+SSDNERF_API int ssdnerf_png_encode_views(const float* pred, const float* real, uint32_t n, uint32_t h, uint32_t w_view, void* workspace,
+                                        size_t workspace_bytes, uint8_t* out, size_t out_bytes, unsigned long long* offsets,
+                                        void* stream);
+/* 2-D maps fp32 [n][h][w] through viridis as matplotlib's Normalize(vmin, vmax) + Colormap(N = 256): index float32((x - vmin) / vrange)
+ * * 256, 256 -> 255, below 0 -> 0, 256 and above -> 255, else truncated; NaN -> (0, 0, 0, 0); vrange = vmax - vmin >= 0 (0: index 0) */
+SSDNERF_API int ssdnerf_png_encode_maps(const float* maps, uint32_t n, uint32_t h, uint32_t w, float vmin, float vrange, void* workspace,
+                                       size_t workspace_bytes, uint8_t* out, size_t out_bytes, unsigned long long* offsets,
+                                       void* stream);
+/* host copy of the viridis table the colormap mode uses, rgb_host [256][3] */
+SSDNERF_API int ssdnerf_png_viridis(uint8_t* rgb_host);
+
 #ifdef __cplusplus
 }
 #endif

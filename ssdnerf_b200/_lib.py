@@ -78,6 +78,15 @@ def lib():
         L.ssdnerf_mc_count.argtypes = [c_void_p, c_u32, c_u32, c_u32, c_double, c_void_p, c_void_p, c_void_p]
         L.ssdnerf_mc_emit.argtypes = [c_void_p, c_u32, c_u32, c_u32, c_double, c_void_p, c_void_p, c_void_p, c_void_p]
         L.ssdnerf_mc_case_table.argtypes = [c_void_p, c_void_p]
+        # PNG encoding (header section 8)
+        for name in ('ssdnerf_png_workspace_bytes', 'ssdnerf_png_output_bound'):
+            getattr(L, name).argtypes = [c_u32, c_u32, c_u32]
+            getattr(L, name).restype = c_size_t
+        L.ssdnerf_png_encode_views.argtypes = [c_void_p, c_void_p, c_u32, c_u32, c_u32, c_void_p, c_size_t, c_void_p, c_size_t,
+                                               c_void_p, c_void_p]
+        L.ssdnerf_png_encode_maps.argtypes = [c_void_p, c_u32, c_u32, c_u32, c_f32, c_f32, c_void_p, c_size_t, c_void_p, c_size_t,
+                                              c_void_p, c_void_p]
+        L.ssdnerf_png_viridis.argtypes = [c_void_p]
         _lib = L
     return _lib
 

@@ -11,11 +11,14 @@ train mode: decoder of the shipped-config shape -> fused differentiable renderer
 code (guidance / code optimisation with a frozen decoder, diffusion_nerf.py:273) and, when the decoder is trainable (stage-1
 auto-decoder training, multiscene_nerf.py:159-252), w.r.t. its weights.  `point_decode` / `point_density_decode` are one native launch (csrc/point_decode.cu).
 """
+import os
+
 import torch
 import torch.nn as nn
 
 from . import _lib as N
 from . import renderer as R
+from . import viz as V
 from .activation import TruncExp
 from .registry import MODULES, build_module
 from .shencoder import SHEncoder
@@ -193,6 +196,12 @@ class TriPlaneDecoder(VolumeRenderer):
         """triplane_decoder.py:181-184"""
         sigmas, _, counts = self.point_decode(xyzs, None, code, density_only=True, **kwargs)
         return sigmas, counts
+
+    def visualize(self, code, scene_name, viz_dir, code_range=[-1, 1]):
+        """triplane_decoder.py:186-194: scene_<name>.png per scene, the code [n, 3, C, h, w] as a [3 h, C w] viridis map over
+        code_range (ssdnerf_b200/viz.py)"""
+        maps = V.code_maps(code.detach().float(), self.flip_z)
+        V.write_pngs([os.path.join(viz_dir, 'scene_' + s + '.png') for s in scene_name], maps=maps, vmin=code_range[0], vmax=code_range[1])
 
     # ------------------------------------------------------------------ forward
     def forward(self, rays_o, rays_d, code, density_bitfield, grid_size, dt_gamma=0, perturb=False, T_thresh=1e-4, return_loss=False):

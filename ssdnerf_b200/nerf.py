@@ -27,6 +27,7 @@ from . import density as D
 from . import mesh as MC
 from . import metrics as M
 from . import renderer as R
+from . import viz as V
 from .registry import MODELS, MODULES, build_module
 from .scene_cache import SceneCache, restore_optimizer_state
 
@@ -544,25 +545,50 @@ class BaseNeRF(nn.Module):
         """base_nerf.py:535-673: render, clamp, 8-bit rounding -> `pred_imgs`.  With `test_imgs` in `data` the log holds `test_psnr`
         (metrics.py:52-55), `test_ssim` (skimage's SSIM, `metrics.ssim`) and, when `use_lpips_metric` is on and LPIPS weights are available
         (`self.lpips`, see ssdnerf_b200/lpips.py), `test_lpips`: means over all scenes and views.  Without weights `test_lpips` is left out
-        with one warning.  Image files under `viz_dir` (matplotlib / mmcv) are not written."""
+        with one warning.  With `viz_dir` (or cfg['viz_dir']) the reference's PNG files are written there (ssdnerf_b200/viz.py): one per
+        view, real | prediction when `test_imgs` are given (named from the per-image metrics, after deleting that view's older files),
+        then `decoder.visualize` of the codes and of `init_code` as `000_mean`."""
         h, w = cfg['img_size']
         image, depth = self.render(decoder, code, density_bitfield, h, w, data['test_intrinsics'], data['test_poses'], cfg=cfg)
         num_scenes, num_imgs = image.shape[:2]
         pred_imgs = image.permute(0, 1, 4, 2, 3).reshape(num_scenes * num_imgs, 3, h, w).clamp(min=0, max=1)
         pred_imgs = torch.round(pred_imgs * 255) / 255
         log_vars = dict()
+        psnr = ssim = lpips = None
         if data.get('test_imgs') is not None:
             target = data['test_imgs'].permute(0, 1, 4, 2, 3).reshape(num_scenes * num_imgs, 3, h, w)
             mse = (pred_imgs - target).square().flatten(1).mean(dim=1)
-            log_vars.update(test_psnr=float((-10 * torch.log10(mse + 1e-6)).mean()))          # eval_psnr (lib/core/evaluation/metrics.py:52-55): eps 1e-6
+            psnr = -10 * torch.log10(mse + 1e-6)          # eval_psnr (lib/core/evaluation/metrics.py:52-55): eps 1e-6
+            log_vars.update(test_psnr=float(psnr.mean()))
             # channels-last views of the same values for the kernels: pred_imgs keeps `image`'s memory order, so this permute copies nothing
             pred_cl = pred_imgs.permute(0, 2, 3, 1).contiguous()
             target_cl = data['test_imgs'].reshape(num_scenes * num_imgs, h, w, 3).contiguous()
-            log_vars.update(test_ssim=float(M.ssim(pred_cl, target_cl).mean()))
+            ssim = M.ssim(pred_cl, target_cl)
+            log_vars.update(test_ssim=float(ssim.mean()))
             lp = self._lpips_metric()
             if lp is not None:
-                log_vars.update(test_lpips=float(lp(pred_cl, target_cl).mean()))
+                lpips = lp(pred_cl, target_cl)
+                log_vars.update(test_lpips=float(lpips.mean()))
+        if viz_dir is None:
+            viz_dir = cfg.get('viz_dir', None)
+        if viz_dir is not None:
+            self._write_viz(viz_dir, data, decoder, code, image, psnr, ssim, lpips, cfg)
         return log_vars, pred_imgs.reshape(num_scenes, num_imgs, 3, h, w)
+
+    def _write_viz(self, viz_dir, data, decoder, code, image, psnr, ssim, lpips, cfg):
+        """base_nerf.py:574-608 on the device encoder: view files, then the triplane maps"""
+        num_scenes, num_imgs, h, w, _ = image.shape
+        os.makedirs(viz_dir, exist_ok=True)
+        test_imgs = data.get('test_imgs') if not cfg.get('skip_eval', False) else None      # base_nerf.py:542: skip_eval -> no real half
+        names, bases = V.view_file_names(data['scene_name'], num_imgs, data.get('test_img_paths') if test_imgs is not None else None,
+                                         None if psnr is None else psnr.tolist(), None if ssim is None else ssim.tolist(),
+                                         None if lpips is None else lpips.tolist())
+        real = None if test_imgs is None else test_imgs.reshape(num_scenes * num_imgs, h, w, 3)
+        V.write_view_files(viz_dir, names, bases, V.encode_png(pred=image.reshape(num_scenes * num_imgs, h, w, 3), real=real))
+        code_range = cfg.get('clip_range', [-1, 1])
+        decoder.visualize(code, data['scene_name'], viz_dir, code_range=code_range)
+        if self.init_code is not None:
+            decoder.visualize(self.init_code[None], ['000_mean'], viz_dir, code_range=code_range)
 
     def mean_ema_update(self, code):
         if self.init_code is None:
@@ -1014,6 +1040,11 @@ class DiffusionNeRF(MultiSceneNeRF):
                 log_vars, pred_imgs = self.eval_and_viz(data, decoder, code, density_bitfield, viz_dir=viz_dir, cfg=self.test_cfg)
             else:
                 log_vars, pred_imgs = dict(), None
+                if viz_dir is None:
+                    viz_dir = self.test_cfg.get('viz_dir', None)
+                if viz_dir is not None:          # diffusion_nerf.py:442-451: the sampled codes' triplane maps alone
+                    os.makedirs(viz_dir, exist_ok=True)
+                    decoder.visualize(code, data['scene_name'], viz_dir, code_range=self.test_cfg.get('clip_range', [-1, 1]))
         save_dir = self.test_cfg.get('save_dir', None)
         if save_dir is not None:
             self.save_scene(save_dir, code, density_grid, density_bitfield, data['scene_name'])
