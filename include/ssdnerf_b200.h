@@ -348,12 +348,14 @@ SSDNERF_API int ssdnerf_col2im_s2(const void* dcol, uint32_t B, uint32_t H, uint
 SSDNERF_API int ssdnerf_sum2x2(const void* dup, uint32_t B, uint32_t H, uint32_t W, uint32_t C, void* dx, void* stream);
 /* dst += src over n fp16 elements (n % 8 == 0) */
 SSDNERF_API int ssdnerf_add_f16(void* dst, const void* src, unsigned long long n, void* stream);
-/* loss scale of an incoming gradient: scale[0] = target / max|g| (1 when g == 0), scale[1] = 1 / scale[0]; g fp32 [n] */
+/* loss scale of an incoming gradient, scale fp32 [4]: scale[0] = target / max|g| (1 when g == 0 or g holds a non-finite value),
+ * scale[1] = 1 / scale[0], scale[2] = 1 when g holds a non-finite value (else 0), scale[3] = 0; g fp32 [n] */
 SSDNERF_API int ssdnerf_grad_scale(const float* g, unsigned long long n, float target, float* scale, void* stream);
-/* g fp32 [B][C][H][W] * scale[0] -> fp16 [B][H][W][Cpad];  dx fp32 [B][H][W][Cpad] * scale[1] -> fp32 [B][C][H][W] */
+/* g fp32 [B][C][H][W] * scale[0] -> fp16 [B][H][W][Cpad];  dx fp32 [B][H][W][Cpad] * scale[1] -> fp32 [B][C][H][W], setting scale[3] = 1
+ * when a result is not finite (the fp16 backward overflowed its headroom, or g was non-finite: scale[2]) */
 SSDNERF_API int ssdnerf_grad_nchw_to_nhwc_f16(const float* g, uint32_t B, uint32_t C, uint32_t H, uint32_t W, uint32_t Cpad, const float* scale,
                                               void* out, void* stream);
-SSDNERF_API int ssdnerf_grad_nhwc_to_nchw_f32(const float* dx, uint32_t B, uint32_t C, uint32_t H, uint32_t W, uint32_t Cpad, const float* scale,
+SSDNERF_API int ssdnerf_grad_nhwc_to_nchw_f32(const float* dx, uint32_t B, uint32_t C, uint32_t H, uint32_t W, uint32_t Cpad, float* scale,
                                               float* out, void* stream);
 
 

@@ -261,19 +261,26 @@ __global__ void k_add_f16(__half* __restrict__ dst, const __half* __restrict__ s
     reinterpret_cast<uint4*>(dst)[i] = bf_to_h8(a);
 }
 
-// loss scale: scale[0] = target / max|g| (1 if g == 0), scale[1] = 1 / scale[0]
+// loss scale: scale[0] = target / max|g| (1 if g == 0 or g holds a non-finite value), scale[1] = 1 / scale[0];
+// scale[2] = 1 if g holds a non-finite value, else 0; scale[3] = 0 (set to 1 by k_grad_nhwc_to_nchw on a non-finite d x)
 __global__ void __launch_bounds__(1024) k_grad_scale(const float* __restrict__ g, size_t n, float target, float* __restrict__ scale) {
     __shared__ float red[32];
     float m = 0.0f;
-    for (size_t i = threadIdx.x; i < n; i += blockDim.x) m = fmaxf(m, fabsf(__ldg(g + i)));
+    bool bad = false;
+    for (size_t i = threadIdx.x; i < n; i += blockDim.x) {
+        const float v = __ldg(g + i);
+        m = fmaxf(m, fabsf(v));             // fmaxf drops a NaN operand: NaN is caught by `bad`
+        bad |= !isfinite(v);
+    }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
     if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
-    __syncthreads();
+    bad = __syncthreads_or(bad);
     if (threadIdx.x == 0) {
         for (int w = 1; w < 32; ++w) m = fmaxf(m, red[w]);
-        const float s = (m > 0.0f && isfinite(m)) ? target / m : 1.0f;
+        const float s = (m > 0.0f && !bad) ? target / m : 1.0f;
         scale[0] = s; scale[1] = 1.0f / s;
+        scale[2] = bad ? 1.0f : 0.0f; scale[3] = 0.0f;
     }
 }
 
@@ -296,15 +303,18 @@ __global__ void k_grad_nchw_to_nhwc(const float* __restrict__ g, uint32_t B, uin
     reinterpret_cast<uint4*>(out)[i] = bf_to_h8(f);
 }
 
-// dx fp32 [B,HW,Cpad] * scale[1] -> fp32 [B,C,H,W]
-__global__ void k_grad_nhwc_to_nchw(const float* __restrict__ dx, uint32_t B, uint32_t C, uint32_t HW, uint32_t Cpad, const float* __restrict__ scale,
+// dx fp32 [B,HW,Cpad] * scale[1] -> fp32 [B,C,H,W]; a non-finite result sets scale[3] = 1 (the fp16 backward overflowed, or g was
+// non-finite: scale[2] tells the two apart)
+__global__ void k_grad_nhwc_to_nchw(const float* __restrict__ dx, uint32_t B, uint32_t C, uint32_t HW, uint32_t Cpad, float* __restrict__ scale,
                                     float* __restrict__ out) {
     const size_t i = threadIdx.x + (size_t)blockIdx.x * blockDim.x;   // over B*C*HW
     if (i >= (size_t)B * C * HW) return;
     const uint32_t pix = (uint32_t)(i % HW);
     const size_t bc = i / HW;
     const uint32_t c = (uint32_t)(bc % C), b = (uint32_t)(bc / C);
-    out[i] = __ldg(dx + ((size_t)b * HW + pix) * Cpad + c) * __ldg(scale + 1);
+    const float v = __ldg(dx + ((size_t)b * HW + pix) * Cpad + c) * scale[1];
+    out[i] = v;
+    if (!isfinite(v)) scale[3] = 1.0f;
 }
 
 }  // namespace ssdnerf
@@ -415,7 +425,7 @@ int ssdnerf_grad_nchw_to_nhwc_f16(const float* g, uint32_t B, uint32_t C, uint32
     return 0;
 }
 
-int ssdnerf_grad_nhwc_to_nchw_f32(const float* dx, uint32_t B, uint32_t C, uint32_t H, uint32_t W, uint32_t Cpad, const float* scale, float* out,
+int ssdnerf_grad_nhwc_to_nchw_f32(const float* dx, uint32_t B, uint32_t C, uint32_t H, uint32_t W, uint32_t Cpad, float* scale, float* out,
                                   void* stream) {
     const size_t n = (size_t)B * C * H * W;
     if (!n) return 0;

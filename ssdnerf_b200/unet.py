@@ -582,29 +582,59 @@ class UNetEngine:
         self.out_conv['wT'] = U.pack_conv_weight_dgrad(m.out.conv.weight, cout_pad=self.CPAD_IN).to(dev)  # K = 18 -> 64, rows = 128
         self._bwd_packed = True
 
-    def backward_nchw(self, grad_v, wg=None):
+    GRAD_TARGET = 1024.0      # max |d loss / d v| after loss scaling: fp16 storage leaves 65504 / 1024 = 64x headroom inside the walk
+    GRAD_RETRIES = 4          # walks after the first, each with the target divided by another 8 (down to 0.25: 262144x headroom)
+
+    def backward_nchw(self, grad_v, weight_grads=False):
         """grad_v fp32 [B,C,H,W] (d loss / d v) -> d loss / d x_t fp32 [B,C,H,W], for the forward that just ran with save=True.
-        With a `unet_train.WeightGradPass` the same walk also produces the parameter gradients: returns (dx, grads, d_scale_shift)."""
+        weight_grads=True: the same walk also produces the parameter gradients (`unet_train.WeightGradPass`): returns
+        (dx, grads, d_scale_shift).
+        A finite grad_v whose gradients overflow the fp16 storage of the walk (d x_t comes out non-finite) is walked again from the same
+        tape with the loss-scale target divided by 8, up to GRAD_RETRIES times; then the first layer that overflows is named in an error.
+        A non-finite grad_v gives a non-finite result, as in fp32 autograd.  Costs one 8-byte device-to-host read per call."""
+        from .unet_train import WeightGradPass
         B, C, H, W = grad_v.shape
         L, s = N.lib(), N.stream_ptr()
-        scale = self._buf(('bwd', 'scale'), (2,), torch.float32)
-        N.check(L.ssdnerf_grad_scale(N.ptr(grad_v), N.ctypes.c_ulonglong(grad_v.numel()), N.c_f32(1024.0), N.ptr(scale), s))
+        scale = self._buf(('bwd', 'scale'), (4,), torch.float32)
         g_in = self._buf(('bwd', 'g_in'), (B, H, W, self.CPAD_IN))
-        N.check(L.ssdnerf_grad_nchw_to_nhwc_f16(N.ptr(grad_v), N.c_u32(B), N.c_u32(C), N.c_u32(H), N.c_u32(W), N.c_u32(self.CPAD_IN),
-                                                N.ptr(scale), N.ptr(g_in), s))
-        dx = self.backward_nhwc(g_in, wg=wg)
         out = torch.empty(B, self.cin_total, H, W, dtype=torch.float32, device=self.dev)
-        N.check(L.ssdnerf_grad_nhwc_to_nchw_f32(N.ptr(dx), N.c_u32(B), N.c_u32(self.cin_total), N.c_u32(H), N.c_u32(W), N.c_u32(self.CPAD_IN),
-                                                N.ptr(scale), N.ptr(out), s))
+
+        def walk(target, check=False):
+            N.check(L.ssdnerf_grad_scale(N.ptr(grad_v), N.ctypes.c_ulonglong(grad_v.numel()), N.c_f32(target), N.ptr(scale), s))
+            N.check(L.ssdnerf_grad_nchw_to_nhwc_f16(N.ptr(grad_v), N.c_u32(B), N.c_u32(C), N.c_u32(H), N.c_u32(W), N.c_u32(self.CPAD_IN),
+                                                    N.ptr(scale), N.ptr(g_in), s))
+            wg = WeightGradPass(self) if weight_grads else None       # fresh per walk: it accumulates
+            dx = self.backward_nhwc(g_in, wg=wg, check=check)
+            N.check(L.ssdnerf_grad_nhwc_to_nchw_f32(N.ptr(dx), N.c_u32(B), N.c_u32(self.cin_total), N.c_u32(H), N.c_u32(W),
+                                                    N.c_u32(self.CPAD_IN), N.ptr(scale), N.ptr(out), s))
+            return wg
+
+        for k in range(self.GRAD_RETRIES + 1):
+            target = self.GRAD_TARGET / 8 ** k
+            wg = walk(target)
+            grad_v_bad, dx_bad = scale[2:].tolist()
+            if grad_v_bad or not dx_bad:
+                break
+        else:
+            walk(target, check=True)          # raises naming the first layer whose gradient is not finite
+            raise N.SSDNeRFNativeError(f'UNet backward: d x_t is not finite at loss-scale target {target} although d loss / d v is')
         if wg is not None:
             grads, d_ss = wg.finish(scale[1])
             return out, grads, d_ss
         return out
 
-    def backward_nhwc(self, g_v, wg=None):
+    def _layer_name(self, r):
+        if r['kind'] == 'out':
+            return 'out'
+        if r['kind'] == 'conv_in':
+            return 'in_blocks.0.0'
+        return next(n for n, mod in self.m.named_modules() if mod is r['d']['mod'])
+
+    def backward_nhwc(self, g_v, wg=None, check=False):
         """g_v fp16 [B,H,W,CPAD_IN] (loss-scaled d loss / d v, zero beyond the model's channels) -> fp32 [B,H,W,CPAD_IN] d loss / d x_in.
         Walks the tape of the last save=True forward in reverse; every convolution / linear gradient is the forward's tensor-core
-        kernel on transposed weights, the rest are the section-4b glue kernels."""
+        kernel on transposed weights, the rest are the section-4b glue kernels.  check=True (diagnosis, synchronises per layer): raise
+        naming the first layer of the walk after which a gradient is not finite."""
         if not self.tape or self.tape[-1]['kind'] != 'out':
             raise N.SSDNeRFNativeError('UNet backward needs a preceding forward_nhwc(save=True)')
         if not self._bwd_packed:
@@ -712,6 +742,9 @@ class UNetEngine:
                     wg.conv_in(r, g)
                 dx_in = self._buf(('bwd', 'dx_in'), (self.B, self.H, self.W, self.CPAD_IN), torch.float32)
                 U.conv3x3_f16(g, self.conv_in['wT'], self.cin_total, out=dx_in, narrow=nw)
+            if check and not all(bool(torch.isfinite(t).all()) for t in list(grads.values()) + ([dx_in] if dx_in is not None else [])):
+                raise N.SSDNeRFNativeError(f'UNet backward: the fp16 gradients overflow at layer `{self._layer_name(r)}` even with the '
+                                           f'loss scale lowered {8 ** self.GRAD_RETRIES}x (forward activations or weights out of range?)')
         assert not grads, 'dangling gradients in the UNet tape'
         return dx_in
 

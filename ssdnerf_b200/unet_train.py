@@ -209,8 +209,7 @@ class _UNetFullGrad(torch.autograd.Function):
         eng = ctx.eng
         if eng.fwd_token != ctx.token:
             raise RuntimeError('UNet gradient: the engine ran another forward before this backward (activations overwritten)')
-        wg = WeightGradPass(eng)
-        dx, grads, d_ss = eng.backward_nchw(grad_v.contiguous().float(), wg=wg)
+        dx, grads, d_ss = eng.backward_nchw(grad_v.contiguous().float(), weight_grads=True)
         live = [p for p in ctx.params if p.requires_grad and p not in grads]
         emb_params = [p for p in live if ctx.ss.requires_grad]
         if emb_params:

@@ -96,11 +96,12 @@ def test_colsum_dropout_and_channel_sums(cuda):
     assert _rel_l2(torch.cat([gamma.detach() * r2 + beta.detach() * r1, r1], dim=1), rss) < 2e-3
 
 
-def _weight_grad_case(cfg, spec, sd, B, res, cuda, oracle_device, bar_each, bar_all):
+def _weight_grad_case(cfg, spec, sd, B, res, cuda, oracle_device, bar_each, bar_all, r=None):
     from ssdnerf_b200.unet import DenoisingUnetMod
     g = torch.Generator().manual_seed(21)
     x = torch.randn(B, 18, res, res, generator=g)
-    r = torch.randn(B, 18, res, res, generator=g) * 1e-3
+    if r is None:
+        r = torch.randn(B, 18, res, res, generator=g) * 1e-3
     t = torch.tensor([999, 400, 19][:B])
     m = DenoisingUnetMod(**cfg)
     m.load_state_dict(sd, strict=True)
