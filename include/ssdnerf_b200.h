@@ -487,6 +487,49 @@ SSDNERF_API int ssdnerf_png_encode_maps(const float* maps, uint32_t n, uint32_t 
 /* host copy of the viridis table the colormap mode uses, rgb_host [256][3] */
 SSDNERF_API int ssdnerf_png_viridis(uint8_t* rgb_host);
 
+/* ------------------------------------------------------------------------------------------------
+ * 9. PNG decoding of dataset views (csrc/png_decode.cu): 8-bit, non-interlaced, colour types 0 / 2 / 3 / 4 / 6.
+ *    replaces: mmcv.imread(path, channel_order='rgb') -> cv2.imread(path, IMREAD_COLOR) and astype(np.float32) / 255 in
+ *              lib/datasets/shapenet_srn.py (parse_scene).
+ *    The host parses the chunks (signature, CRCs, IHDR, PLTE, IDAT) and passes each image's zlib stream: its IDAT payloads
+ *    concatenated.  Output float32 [h][w][3] RGB per image, value = byte / 255 (IEEE division): grey replicated, palette expanded,
+ *    alpha dropped, tRNS ignored, as cv2's IMREAD_COLOR.  Each image gets a status (SSDNERF_PNG_*); a malformed stream never
+ *    reads past its `stream_bytes`, never writes past its workspace slice or output, and leaves its output undefined.
+ * ---------------------------------------------------------------------------------------------- */
+#define SSDNERF_PNG_OK 0
+#define SSDNERF_PNG_TRUNCATED 1          /* the stream ends before the deflate data or the Adler-32 does */
+#define SSDNERF_PNG_BAD_ZLIB_HEADER 2    /* CM != 8, window > 32 K, FCHECK fails or FDICT set */
+#define SSDNERF_PNG_BAD_BLOCK_TYPE 3     /* block type 3 */
+#define SSDNERF_PNG_BAD_STORED_LEN 4     /* stored block with LEN != ~NLEN */
+#define SSDNERF_PNG_BAD_CODE_LENGTHS 5   /* over-subscribed or incomplete code, a bad repeat, too many symbols, no end-of-block code */
+#define SSDNERF_PNG_BAD_SYMBOL 6         /* a bit pattern with no code, or literal / length 286-287, distance 30-31 */
+#define SSDNERF_PNG_BAD_DISTANCE 7       /* a match reaching before the first byte */
+#define SSDNERF_PNG_TOO_MUCH_DATA 8      /* more than h (1 + w bpp) bytes */
+#define SSDNERF_PNG_TOO_LITTLE_DATA 9    /* the last block ends short of h (1 + w bpp) bytes */
+#define SSDNERF_PNG_BAD_FILTER 10        /* a row filter type above 4 */
+#define SSDNERF_PNG_BAD_ADLER 11         /* Adler-32 mismatch */
+#define SSDNERF_PNG_BAD_DESC 12          /* the descriptor's ranges leave the buffers, or its size / colour type is unsupported */
+typedef struct {
+    uint64_t stream_offset;   /* bytes into `streams`: the image's zlib stream */
+    uint64_t palette_offset;  /* bytes into `streams`: 768 bytes, the PLTE entries zero-padded to 256 (colour type 3 only) */
+    uint64_t work_offset;     /* bytes into `workspace`: ssdnerf_png_decode_workspace_bytes(h, w, color_type) of them */
+    uint64_t out_offset;      /* floats into `out`: h * w * 3 of them */
+    uint32_t stream_bytes;
+    uint32_t h, w;
+    int32_t color_type;
+} ssdnerf_png_desc;
+/* scratch bytes (a multiple of 16) for one h x w image: its inflated, filtered stream; 0 for a zero size, an unsupported colour type,
+ * or h (1 + w bpp) >= 2^31 */
+SSDNERF_API size_t ssdnerf_png_decode_workspace_bytes(uint32_t h, uint32_t w, int color_type);
+/* decodes n images (one warp each): desc device [n] (8-byte aligned), out fp32, status int32 [n].  Nothing synchronises: read the
+ * statuses after the stream completes. */
+SSDNERF_API int ssdnerf_png_decode(const uint8_t* streams, size_t stream_bytes, const ssdnerf_png_desc* desc, uint32_t n, void* workspace,
+                                   size_t workspace_bytes, float* out, size_t out_floats, int32_t* status, void* stream);
+/* the same decode and validation of one image on the CPU (host pointers; scratch allocated internally): out_host fp32 [h][w][3],
+ * *status_host the image's status.  Returns SSDNERF_ERR_ARG for missing pointers or a size the workspace query refuses. */
+SSDNERF_API int ssdnerf_png_decode_host(const uint8_t* stream_host, size_t stream_bytes, uint32_t h, uint32_t w, int color_type,
+                                        const uint8_t* palette_host, float* out_host, int32_t* status_host);
+
 #ifdef __cplusplus
 }
 #endif

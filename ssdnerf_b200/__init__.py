@@ -6,12 +6,14 @@
     raymarching / shencoder / activation : one-to-one mirrors of the reference's lib.ops (csrc/legacy_ops.cu)
     mesh                : marching cubes + binary STL of save_mesh  (csrc/mesh.cu)
     viz                 : PNG files under viz_dir, interpolation demo (csrc/png.cu)
+    datasets            : ShapeNet SRN scenes, GPU PNG decoding of their views (csrc/png_decode.cu)
 
 Everything computes through libssdnerf_b200.so (C ABI: include/ssdnerf_b200.h); there is no CPU or PyTorch fallback.
 """
-from .registry import MODELS, MODULES, build_model, build_module  # noqa: F401
+from .registry import DATASETS, MODELS, MODULES, build_dataset, build_model, build_module  # noqa: F401
 from .config import Config  # noqa: F401
-from . import activation, decoders, density, diffusion, mesh, nerf, raymarching, renderer, scene_cache, shencoder, unet, viz  # noqa: F401
+from . import activation, datasets, decoders, density, diffusion, mesh, nerf, raymarching, renderer, scene_cache, shencoder, unet, viz  # noqa: F401
+from .datasets import ShapeNetSRN, collate, decode_png  # noqa: F401
 from .decoders import TriPlaneDecoder  # noqa: F401
 from .diffusion import GaussianDiffusion  # noqa: F401
 from .nerf import DiffusionNeRF, MultiSceneNeRF  # noqa: F401

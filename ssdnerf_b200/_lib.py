@@ -87,6 +87,11 @@ def lib():
         L.ssdnerf_png_encode_maps.argtypes = [c_void_p, c_u32, c_u32, c_u32, c_f32, c_f32, c_void_p, c_size_t, c_void_p, c_size_t,
                                               c_void_p, c_void_p]
         L.ssdnerf_png_viridis.argtypes = [c_void_p]
+        # PNG decoding (header section 9)
+        L.ssdnerf_png_decode_workspace_bytes.argtypes = [c_u32, c_u32, c_int]
+        L.ssdnerf_png_decode_workspace_bytes.restype = c_size_t
+        L.ssdnerf_png_decode.argtypes = [c_void_p, c_size_t, c_void_p, c_u32, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p, c_void_p]
+        L.ssdnerf_png_decode_host.argtypes = [ctypes.c_char_p, c_size_t, c_u32, c_u32, c_int, ctypes.c_char_p, c_void_p, c_void_p]
         _lib = L
     return _lib
 

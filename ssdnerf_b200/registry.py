@@ -2,7 +2,7 @@
 
 The reference registers its classes into mmgen's ``MODELS`` / ``MODULES`` registries and builds them from
 config dicts with ``build_module`` (mmgen/models/builder.py).  mmcv / mmgen are not installable offline, so this
-module provides the same two registries and builder semantics (``type`` key, ``default_args``), and, when the real
+module provides the same registries (and ``DATASETS``) and builder semantics (``type`` key, ``default_args``), and, when the real
 mmgen IS importable, additionally registers every class there so the reference's own ``build_model`` finds them.
 """
 import inspect
@@ -37,7 +37,10 @@ class Registry:
 
 def _mirror_to_mmgen(registry_name, key, cls):
     try:   # pragma: no cover - mmgen is absent in the build container
-        from mmgen.models import builder as mb
+        if registry_name == 'datasets':
+            from mmgen.datasets import builder as mb
+        else:
+            from mmgen.models import builder as mb
         reg = getattr(mb, registry_name.upper(), None)
         if reg is not None and key not in reg.module_dict:
             reg.register_module(name=key, module=cls)
@@ -67,6 +70,7 @@ def build_from_cfg(cfg, registry, default_args=None):
 
 MODELS = Registry('models')
 MODULES = Registry('modules')
+DATASETS = Registry('datasets')
 
 
 def build_module(cfg, default_args=None):
@@ -79,3 +83,8 @@ def build_module(cfg, default_args=None):
 def build_model(cfg, train_cfg=None, test_cfg=None):
     """mmgen.models.builder.build_model"""
     return build_from_cfg(cfg, MODELS, dict(train_cfg=train_cfg, test_cfg=test_cfg))
+
+
+def build_dataset(cfg, default_args=None):
+    """mmgen.datasets.build_dataset for a single dataset dict (ssdnerf_b200.datasets registers ShapeNetSRN)"""
+    return build_from_cfg(cfg, DATASETS, default_args)
