@@ -302,9 +302,9 @@ int ssdnerf_density_update(int variant, const void* planes, uint32_t plane_h, ui
     const bool is_s = variant == SSDNERF_DEC_S;
     if (!is_s && variant != SSDNERF_DEC_P)
         return set_error_msg(SSDNERF_ERR_ARG, "density_update: unknown decoder variant");
-    if (!planes || !decoder_blob || !density_grid || !workspace) return set_error_msg(SSDNERF_ERR_ARG, "density_update: NULL argument");
     if (grid_size == 0 || grid_size > 1024 || (grid_size & (grid_size - 1))) return set_error_msg(SSDNERF_ERR_ARG, "density_update: grid_size must be a power of two");
-    if (num_scenes == 0) return 0;
+    if (num_scenes == 0) return 0;   // before the pointer checks: the tensors of an empty batch have no storage
+    if (!planes || !decoder_blob || !density_grid || !workspace) return set_error_msg(SSDNERF_ERR_ARG, "density_update: NULL argument");
     const size_t total = (size_t)num_scenes * grid_size * grid_size * grid_size;
     float* partials = reinterpret_cast<float*>((unsigned char*)workspace + 16);
     if (is_s) {
@@ -338,8 +338,8 @@ int ssdnerf_density_update(int variant, const void* planes, uint32_t plane_h, ui
 int ssdnerf_density_pack(const void* density_grid, int grid_is_half, uint32_t num_scenes, uint32_t grid_size, float density_thresh,
                          uint8_t* bitfield, float* thresh_out, void* workspace, void* stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
-    if (!density_grid || !bitfield || !workspace) return set_error_msg(SSDNERF_ERR_ARG, "density_pack: NULL argument");
     if (num_scenes == 0) return 0;
+    if (!density_grid || !bitfield || !workspace) return set_error_msg(SSDNERF_ERR_ARG, "density_pack: NULL argument");
     const size_t total = (size_t)num_scenes * grid_size * grid_size * grid_size;
     const uint32_t blocks = (uint32_t)((total + kDenThreads - 1) / kDenThreads);
     float* thresh = reinterpret_cast<float*>(workspace);
