@@ -530,6 +530,88 @@ SSDNERF_API int ssdnerf_png_decode(const uint8_t* streams, size_t stream_bytes, 
 SSDNERF_API int ssdnerf_png_decode_host(const uint8_t* stream_host, size_t stream_bytes, uint32_t h, uint32_t w, int color_type,
                                         const uint8_t* palette_host, float* out_host, int32_t* status_host);
 
+/* ------------------------------------------------------------------------------------------------
+ * 10. KITTI instance crops (csrc/kitti.cu, csrc/png_decode.cu, csrc/png.cu).
+ *     replaces: tools/kitti_preproc.py (mmcv.imread(..., 'unchanged'), the mask / whitening / np.pad / mmcv.imresize of each
+ *               instance, mmcv.imwrite).
+ *     Raw decode: 8-bit grey (colour type 0), 8-bit RGB (2) and 16-bit grey as cv2.imread(IMREAD_UNCHANGED): u8 samples in BGR
+ *     order, or native-endian uint16; statuses as section 9.  Boxes: per (frame, label line i) the pixels equal to 1000 + i.
+ *     Crops: the whitened crop of each kept instance and its out_size^2 view (pad to a white square, cv2.resize INTER_LINEAR,
+ *     white border), where a box pixel is 255 when its value is not the instance's or when an earlier whitening instance of the
+ *     frame has it in its box (the reference whitens through a view into the frame, instance by instance).  PNG: BGR u8 images of
+ *     their own sizes written as 8-bit RGB (colour type 2) files, as cv2.imwrite does; the contract is the decoded pixels.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct {
+    uint64_t stream_offset;   /* bytes into `streams`: the image's zlib stream (its IDAT payloads concatenated) */
+    uint64_t work_offset;     /* bytes into `workspace`: ssdnerf_png_decode_raw_workspace_bytes(...) of them */
+    uint64_t out_offset;      /* bytes into `out`: h * w * bytes per pixel (1, 3 or 2) of them */
+    uint32_t stream_bytes;
+    uint32_t h, w;
+    int32_t color_type;       /* 0 or 2 at bit depth 8; 0 at bit depth 16 */
+    int32_t bit_depth;
+    uint32_t reserved;
+} ssdnerf_png_raw_desc;
+/* scratch bytes (a multiple of 16) for one image; 0 for an unsupported format or size */
+SSDNERF_API size_t ssdnerf_png_decode_raw_workspace_bytes(uint32_t h, uint32_t w, int color_type, int bit_depth);
+/* decodes n images (one warp each): desc device [n] (8-byte aligned), status int32 [n]; nothing synchronises */
+SSDNERF_API int ssdnerf_png_decode_raw(const uint8_t* streams, size_t stream_bytes, const ssdnerf_png_raw_desc* desc, uint32_t n,
+                                       void* workspace, size_t workspace_bytes, uint8_t* out, size_t out_bytes, int32_t* status,
+                                       void* stream);
+/* the same decode of one image on the CPU: out_host [h][w][bytes per pixel], *status_host its status */
+SSDNERF_API int ssdnerf_png_decode_raw_host(const uint8_t* stream_host, size_t stream_bytes, uint32_t h, uint32_t w, int color_type,
+                                            int bit_depth, uint8_t* out_host, int32_t* status_host);
+
+#define SSDNERF_KITTI_MAX_LABELS 1024   /* label lines per frame the box pass takes */
+typedef struct {
+    uint64_t seg_offset;      /* uint16 elements into `seg`: the frame's instance map [h][w] */
+    uint32_t h, w;
+    uint32_t box_offset;      /* the frame's first record in `boxes` */
+    uint32_t num_labels;      /* label lines: record box_offset + i counts the value 1000 + i */
+} ssdnerf_kitti_frame;
+/* boxes int32 [sum num_labels][5] = (pixel count, y_min, y_max + 1, x_min, x_max + 1); the box fields are undefined at count 0.
+ * frames device [n] (8-byte aligned). */
+SSDNERF_API int ssdnerf_kitti_boxes(const uint16_t* seg, const ssdnerf_kitti_frame* frames, uint32_t n, int32_t* boxes,
+                                    uint32_t num_boxes, void* stream);
+
+typedef struct {
+    uint64_t image_offset;    /* bytes into `images`: the frame, BGR u8 [frame_h][frame_w][3] */
+    uint64_t seg_offset;      /* uint16 elements into `seg`: its instance map [frame_h][frame_w] */
+    uint64_t crop_offset;     /* bytes into `crops`: the whitened crop, BGR u8 [h][w][3] */
+    uint64_t view_offset;     /* bytes into `views`: the view, BGR u8 [out_size][out_size][3] */
+    uint32_t frame_w;
+    uint32_t y0, x0, h, w;    /* the instance's box in the frame */
+    uint32_t label;           /* the instance's value in the map (1000 + label line) */
+    uint32_t pad_tgt;         /* side of the white square, >= max(h, w) and >= out_size - 2 out_border */
+    uint32_t pad_y, pad_x;    /* the box's offset in the square: (pad_tgt - h) / 2, (pad_tgt - w) / 2 */
+    uint32_t prior_first;     /* the earlier whitening instances of the frame: records prior_first .. + prior_count of `priors`, */
+    uint32_t prior_count;     /*   each int32 (y_min, y_max + 1, x_min, x_max + 1, value) */
+} ssdnerf_kitti_crop;
+/* one launch over n crop jobs (desc device [n], 8-byte aligned) */
+SSDNERF_API int ssdnerf_kitti_crops(const uint8_t* images, const uint16_t* seg, const ssdnerf_kitti_crop* desc, uint32_t n,
+                                    const int32_t* priors, uint32_t out_size, uint32_t out_border, uint8_t* crops, uint8_t* views,
+                                    void* stream);
+/* cv2.resize(src, (dw, dh), interpolation=INTER_LINEAR) of a u8 [sh][sw][3] image on the CPU, by the same arithmetic as the views:
+ * OpenCV's 11-bit fixed-point coefficients, the horizontal pass, the vertical pass as its vector path computes it (16-bit products
+ * of the >> 4 sums, then a rounding >> 2), and its 2 x 2 average when the size halves exactly */
+SSDNERF_API int ssdnerf_kitti_resize_host(const uint8_t* src_host, uint32_t sh, uint32_t sw, uint32_t dh, uint32_t dw, uint8_t* dst_host);
+
+typedef struct {
+    uint64_t src_offset;      /* bytes into `images`: BGR u8 [h][w][3] (caller) */
+    uint32_t h, w;            /* (caller) */
+    uint64_t filt_offset;     /* the filtered stream in the workspace (set by ssdnerf_png_bgr_layout) */
+    uint32_t seg_first;       /* the image's first deflate segment (set by ssdnerf_png_bgr_layout) */
+    uint32_t reserved;
+} ssdnerf_png_bgr_desc;
+/* lays out n images (host descriptors with h and w set; rows of 3 w + 1 bytes at most SSDNERF_PNG_SEGMENT_BYTES) in the workspace:
+ * images of one size are adjacent, so each size is deflated by one grid.  *workspace_bytes: the workspace the encode needs;
+ * *output_bound: the largest total the n files can take. */
+SSDNERF_API int ssdnerf_png_bgr_layout(ssdnerf_png_bgr_desc* desc_host, uint32_t n, size_t* workspace_bytes, size_t* output_bound);
+/* encodes n laid-out images into files out[offsets[i] : offsets[i + 1]] (offsets uint64 [n + 1] on the device): desc the descriptors
+ * on the device, desc_host the same on the host (it sizes the launches) */
+SSDNERF_API int ssdnerf_png_encode_bgr(const uint8_t* images, const ssdnerf_png_bgr_desc* desc, const ssdnerf_png_bgr_desc* desc_host,
+                                       uint32_t n, void* workspace, size_t workspace_bytes, uint8_t* out, size_t out_bytes,
+                                       unsigned long long* offsets, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

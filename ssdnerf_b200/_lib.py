@@ -92,6 +92,17 @@ def lib():
         L.ssdnerf_png_decode_workspace_bytes.restype = c_size_t
         L.ssdnerf_png_decode.argtypes = [c_void_p, c_size_t, c_void_p, c_u32, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p, c_void_p]
         L.ssdnerf_png_decode_host.argtypes = [ctypes.c_char_p, c_size_t, c_u32, c_u32, c_int, ctypes.c_char_p, c_void_p, c_void_p]
+        # KITTI instance crops (header section 10)
+        L.ssdnerf_png_decode_raw_workspace_bytes.argtypes = [c_u32, c_u32, c_int, c_int]
+        L.ssdnerf_png_decode_raw_workspace_bytes.restype = c_size_t
+        L.ssdnerf_png_decode_raw.argtypes = [c_void_p, c_size_t, c_void_p, c_u32, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p,
+                                             c_void_p]
+        L.ssdnerf_png_decode_raw_host.argtypes = [ctypes.c_char_p, c_size_t, c_u32, c_u32, c_int, c_int, c_void_p, c_void_p]
+        L.ssdnerf_kitti_boxes.argtypes = [c_void_p, c_void_p, c_u32, c_void_p, c_u32, c_void_p]
+        L.ssdnerf_kitti_crops.argtypes = [c_void_p, c_void_p, c_void_p, c_u32, c_void_p, c_u32, c_u32, c_void_p, c_void_p, c_void_p]
+        L.ssdnerf_kitti_resize_host.argtypes = [c_void_p, c_u32, c_u32, c_u32, c_u32, c_void_p]
+        L.ssdnerf_png_bgr_layout.argtypes = [c_void_p, c_u32, c_void_p, c_void_p]
+        L.ssdnerf_png_encode_bgr.argtypes = [c_void_p, c_void_p, c_void_p, c_u32, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p, c_void_p]
         _lib = L
     return _lib
 

@@ -15,12 +15,17 @@
 // * k_png_sizes / k_png_write: file sizes and offsets (one scan), then per file the signature, IHDR, one IDAT (zlib header, the
 //   segments, runs of stored segments re-cut into stored blocks of up to 65535 bytes, Adler-32 of the filtered stream) with its
 //   CRC-32 from per-thread partials combined by GF(2) shifts, and IEND.
+// * BGR u8 images of their own sizes (header section 10, KITTI crops): k_png_filter_bgr builds 8-bit RGB rows (colour type 2) from
+//   the bytes; images of one size lie next to each other in the workspace, so k_png_deflate runs unchanged once per size;
+//   k_png_sizes_bgr / k_png_write_bgr are the per-file versions of the two last passes.
 // * Determinism: a file's bytes depend only on its pixels.  The only atomics are an integer max into the hash table, integer
 //   frequency counts and ORs into disjoint bit fields, whose results do not depend on their order.
 #include "common.cuh"
 #include "../../include/ssdnerf_b200.h"
 #include <cstdio>
 #include <cstring>
+#include <algorithm>
+#include <vector>
 
 namespace ssdnerf {
 
@@ -747,9 +752,281 @@ static int png_encode(const PngSrc& src, uint32_t n, uint32_t h, uint32_t w, voi
     return 0;
 }
 
+// ------------------------------------------------------------------------------------------------ BGR u8 images of their own sizes
+// one image's geometry at 3 bytes per pixel (the deflate and assembly of one size group read it like png_geom's)
+__host__ __device__ inline PngGeom png_geom_rgb(uint32_t n, uint32_t h, uint32_t w) {
+    PngGeom g;
+    g.n = n; g.h = h; g.w = w;
+    g.rowbytes = 3 * w + 1;
+    g.raw = (uint64_t)h * g.rowbytes;
+    g.rps = g.rowbytes <= (uint32_t)kSegCap ? kSegCap / g.rowbytes : 0;
+    g.nseg = g.rps ? (h + g.rps - 1) / g.rps : 0;
+    return g;
+}
+
+// one warp per row (grid: rows / 8 x images): the row's RGB bytes from BGR, the least-sum filter as k_png_filter picks it
+__global__ void __launch_bounds__(256) k_png_filter_bgr(const uint8_t* __restrict__ images, const ssdnerf_png_bgr_desc* __restrict__ desc,
+                                                        uint8_t* __restrict__ ws) {
+    const ssdnerf_png_bgr_desc d = desc[blockIdx.y];
+    const uint32_t y = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (y >= d.h) return;
+    const uint32_t rowbytes = 3 * d.w + 1;
+    uint8_t* out = ws + d.filt_offset + (uint64_t)y * rowbytes;
+    const uint8_t* src = images + d.src_offset;
+    auto pix = [&](uint32_t yy, uint32_t x) {
+        const uint8_t* p = src + ((uint64_t)yy * d.w + x) * 3;
+        return (uint32_t)p[2] | ((uint32_t)p[1] << 8) | ((uint32_t)p[0] << 16);
+    };
+    uint32_t best = 0;
+    for (int pass = 0; pass < 2; ++pass) {
+        uint32_t sum[5] = {0, 0, 0, 0, 0};
+        uint32_t carry_cur = 0, carry_up = 0;
+        for (uint32_t x0 = 0; x0 < d.w; x0 += 32) {
+            const uint32_t x = x0 + lane;
+            uint32_t cur = 0, up = 0;
+            if (x < d.w) {
+                cur = pix(y, x);
+                up = y ? pix(y - 1, x) : 0u;
+            }
+            uint32_t left = __shfl_up_sync(0xffffffffu, cur, 1), ul = __shfl_up_sync(0xffffffffu, up, 1);
+            if (lane == 0) { left = carry_cur; ul = carry_up; }
+            carry_cur = __shfl_sync(0xffffffffu, cur, 31);
+            carry_up = __shfl_sync(0xffffffffu, up, 31);
+            if (x < d.w) {
+                if (pass == 0) {
+#pragma unroll
+                    for (int k = 0; k < 3; ++k) {
+                        const int xv = (cur >> (8 * k)) & 0xFF, a = (left >> (8 * k)) & 0xFF, b = (up >> (8 * k)) & 0xFF,
+                                  c = (ul >> (8 * k)) & 0xFF;
+#pragma unroll
+                        for (int t = 0; t < 5; ++t) sum[t] += abs((int)(int8_t)filt_byte(t, xv, a, b, c));
+                    }
+                } else {
+#pragma unroll
+                    for (int k = 0; k < 3; ++k)
+                        out[1 + 3 * x + k] = (uint8_t)filt_byte((int)best, (cur >> (8 * k)) & 0xFF, (left >> (8 * k)) & 0xFF,
+                                                                (up >> (8 * k)) & 0xFF, (ul >> (8 * k)) & 0xFF);
+                }
+            }
+        }
+        if (pass == 0) {
+#pragma unroll
+            for (int t = 0; t < 5; ++t)
+                for (int o = 16; o; o >>= 1) sum[t] += __shfl_xor_sync(0xffffffffu, sum[t], o);
+            for (int t = 1; t < 5; ++t)
+                if (sum[t] < sum[best]) best = t;
+            if (lane == 0) out[0] = (uint8_t)best;
+        }
+    }
+}
+
+__device__ __forceinline__ uint64_t bgr_file_bytes(const ssdnerf_png_bgr_desc& d, const uint32_t* seg_info) {
+    return kFileOverhead + deflate_bytes(png_geom_rgb(1, d.h, d.w), seg_info + d.seg_first, 0);
+}
+
+// offsets[i] = first byte of file i, offsets[n] = total (one CTA), as k_png_sizes
+__global__ void __launch_bounds__(1024) k_png_sizes_bgr(const ssdnerf_png_bgr_desc* __restrict__ desc, uint32_t n,
+                                                        const uint32_t* __restrict__ seg_info, unsigned long long* offsets) {
+    __shared__ uint64_t wsum[32];
+    const uint32_t tid = threadIdx.x, per = div_up(n, 1024), f0 = min(tid * per, n), f1 = min(f0 + per, n);
+    uint64_t mine = 0;
+    for (uint32_t f = f0; f < f1; ++f) mine += bgr_file_bytes(desc[f], seg_info);
+    uint64_t incl = mine;
+    for (int o = 1; o < 32; o <<= 1) {
+        const uint64_t t = __shfl_up_sync(0xffffffffu, incl, o);
+        if ((tid & 31) >= (uint32_t)o) incl += t;
+    }
+    if ((tid & 31) == 31) wsum[tid >> 5] = incl;
+    __syncthreads();
+    uint64_t base = 0, total = 0;
+    for (uint32_t k = 0; k < 32; ++k) { if (k < (tid >> 5)) base += wsum[k]; total += wsum[k]; }
+    uint64_t o = base + incl - mine;
+    for (uint32_t f = f0; f < f1; ++f) { offsets[f] = o; o += bgr_file_bytes(desc[f], seg_info); }
+    if (tid == 0) offsets[n] = total;
+}
+
+// one CTA per file, as k_png_write with the file's own geometry and colour type 2
+__global__ void __launch_bounds__(kWriteThreads) k_png_write_bgr(const ssdnerf_png_bgr_desc* __restrict__ desc, const uint8_t* __restrict__ ws,
+                                                                const uint8_t* __restrict__ slots, const uint32_t* __restrict__ seg_info,
+                                                                const unsigned long long* __restrict__ offsets, uint8_t* __restrict__ out) {
+    __shared__ uint32_t tab[256];
+    __shared__ uint32_t pcrc[kWriteThreads];
+    __shared__ uint64_t plen[kWriteThreads], ps1[kWriteThreads], ps2[kWriteThreads];
+    const uint32_t f = blockIdx.x, tid = threadIdx.x;
+    const ssdnerf_png_bgr_desc d = desc[f];
+    const PngGeom g = png_geom_rgb(1, d.h, d.w);
+    tab[tid] = crc_table_entry(tid);
+    uint8_t* o = out + offsets[f];
+    const uint64_t dlen = offsets[f + 1] - offsets[f] - kFileOverhead;
+    const uint8_t* fraw = ws + d.filt_offset;
+    __syncthreads();
+    if (tid == 0) {
+        const uint8_t sig[8] = {0x89, 'P', 'N', 'G', '\r', '\n', 0x1A, '\n'};
+        for (int i = 0; i < 8; ++i) o[i] = sig[i];
+        put_be32(o + 8, 13);
+        o[12] = 'I'; o[13] = 'H'; o[14] = 'D'; o[15] = 'R';
+        put_be32(o + 16, g.w); put_be32(o + 20, g.h);
+        o[24] = 8; o[25] = 2; o[26] = 0; o[27] = 0; o[28] = 0;      // 8-bit RGB, deflate, adaptive filtering, no interlace
+        uint32_t c = 0xFFFFFFFFu;
+        for (int i = 12; i < 29; ++i) c = tab[(c ^ o[i]) & 0xFF] ^ (c >> 8);
+        put_be32(o + 29, ~c);
+        put_be32(o + 33, (uint32_t)(dlen + 6));
+        o[37] = 'I'; o[38] = 'D'; o[39] = 'A'; o[40] = 'T';
+        o[41] = 0x78; o[42] = 0x9C;
+    }
+    const uint32_t* info = seg_info + d.seg_first;
+    uint64_t pos = 43;
+    for (uint32_t s = 0; s < g.nseg;) {
+        if (info[s] != kStored) {
+            const uint8_t* slot = slots + ((uint64_t)d.seg_first + s) * kSlotBytes;
+            for (uint32_t i = tid; i < info[s]; i += kWriteThreads) o[pos + i] = slot[i];
+            pos += info[s++];
+            continue;
+        }
+        const uint32_t s_first = s;
+        uint64_t R = 0;
+        while (s < g.nseg && info[s] == kStored) R += seg_len(g, s++);
+        const uint8_t* src = fraw + seg_start(g, s_first);
+        for (uint64_t done = 0; done < R;) {
+            const uint32_t L = (uint32_t)(R - done < 65535 ? R - done : 65535);
+            if (tid == 0) {
+                o[pos] = (s == g.nseg && done + L == R) ? 1 : 0;
+                o[pos + 1] = (uint8_t)L; o[pos + 2] = (uint8_t)(L >> 8);
+                o[pos + 3] = (uint8_t)~L; o[pos + 4] = (uint8_t)(~L >> 8);
+            }
+            for (uint32_t i = tid; i < L; i += kWriteThreads) o[pos + 5 + i] = src[done + i];
+            pos += 5 + L;
+            done += L;
+        }
+    }
+    {
+        uint64_t s1 = 0, s2 = 0;
+        for (uint64_t i = tid; i < g.raw; i += kWriteThreads) { const uint64_t b = fraw[i]; s1 += b; s2 += ((g.raw - i) % 65521) * b; }
+        ps1[tid] = s1 % 65521; ps2[tid] = s2 % 65521;
+        __syncthreads();
+        if (tid == 0) {
+            uint64_t a = 1, b = g.raw % 65521;
+            for (int k = 0; k < kWriteThreads; ++k) { a += ps1[k]; b += ps2[k]; }
+            put_be32(o + 43 + dlen, (uint32_t)((b % 65521) << 16 | (a % 65521)));
+        }
+    }
+    __syncthreads();
+    const uint64_t L = 4 + dlen + 6, chunk = (L + kWriteThreads - 1) / kWriteThreads;
+    const uint64_t a0 = min(L, tid * chunk), a1 = min(L, a0 + chunk);
+    uint32_t c = 0;
+    for (uint64_t i = a0; i < a1; ++i) c = tab[(c ^ o[37 + i]) & 0xFF] ^ (c >> 8);
+    pcrc[tid] = c; plen[tid] = a1 - a0;
+    __syncthreads();
+    for (uint32_t dd = 1; dd < kWriteThreads; dd <<= 1) {
+        if ((tid & (2 * dd - 1)) == 0 && plen[tid + dd]) {
+            pcrc[tid] = multmodp(crc_shift_op(plen[tid + dd]), pcrc[tid]) ^ pcrc[tid + dd];
+            plen[tid] += plen[tid + dd];
+        }
+        __syncthreads();
+    }
+    if (tid == 0) {
+        const uint32_t crc = ~(multmodp(crc_shift_op(L), 0xFFFFFFFFu) ^ pcrc[0]);
+        put_be32(o + 47 + dlen, crc);
+        const uint8_t iend[12] = {0, 0, 0, 0, 'I', 'E', 'N', 'D', 0xAE, 0x42, 0x60, 0x82};
+        for (int i = 0; i < 12; ++i) o[51 + dlen + i] = iend[i];
+    }
+}
+
+static bool bgr_dims_ok(uint32_t h, uint32_t w) {
+    if (!h || !w) return false;
+    const PngGeom g = png_geom_rgb(1, h, w);
+    return g.rps && g.raw < (1ull << 31);
+}
+
+// the images' order in the workspace: by size (h, then w), stable
+static std::vector<uint32_t> bgr_order(const ssdnerf_png_bgr_desc* d, uint32_t n) {
+    std::vector<uint32_t> ord(n);
+    for (uint32_t i = 0; i < n; ++i) ord[i] = i;
+    std::stable_sort(ord.begin(), ord.end(), [&](uint32_t a, uint32_t b) { return d[a].h != d[b].h ? d[a].h < d[b].h : d[a].w < d[b].w; });
+    return ord;
+}
+
 }  // namespace ssdnerf
 
 using namespace ssdnerf;
+
+extern "C" int ssdnerf_png_bgr_layout(ssdnerf_png_bgr_desc* desc_host, uint32_t n, size_t* workspace_bytes, size_t* output_bound) {
+    if (!desc_host || !workspace_bytes || !output_bound) return set_error_msg(SSDNERF_ERR_ARG, "png_bgr_layout: NULL argument");
+    uint64_t filt = 0, segs = 0, bound = 0;
+    for (uint32_t i : bgr_order(desc_host, n)) {
+        ssdnerf_png_bgr_desc& d = desc_host[i];
+        if (!bgr_dims_ok(d.h, d.w)) {
+            static thread_local char msg[160];
+            snprintf(msg, sizeof(msg), "png_bgr_layout: image %u is %u x %u; h, w >= 1 and a row (3 w + 1 bytes) at most %d bytes", i, d.h, d.w,
+                     kSegCap);
+            return set_error_msg(SSDNERF_ERR_ARG, msg);
+        }
+        const PngGeom g = png_geom_rgb(1, d.h, d.w);
+        d.filt_offset = filt;
+        d.seg_first = (uint32_t)segs;
+        filt += g.raw;
+        segs += g.nseg;
+        bound += kFileOverhead + g.raw + 5ull * g.nseg;
+    }
+    if (segs >= (1ull << 31)) return set_error_msg(SSDNERF_ERR_ARG, "png_bgr_layout: too many segments");
+    *workspace_bytes = align256(filt) + align256(segs * kSlotBytes) + align256(segs * 4);
+    *output_bound = bound;
+    return 0;
+}
+
+extern "C" int ssdnerf_png_encode_bgr(const uint8_t* images, const ssdnerf_png_bgr_desc* desc, const ssdnerf_png_bgr_desc* desc_host,
+                                      uint32_t n, void* workspace, size_t workspace_bytes, uint8_t* out, size_t out_bytes,
+                                      unsigned long long* offsets, void* stream) {
+    if (n == 0) return 0;
+    if (!images || !desc || !desc_host || !workspace || !out || !offsets || ((uintptr_t)desc & 7u) || ((uintptr_t)offsets & 7u) ||
+        ((uintptr_t)workspace & 255u))
+        return set_error_msg(SSDNERF_ERR_ARG, "png_encode_bgr: images, desc (8-byte aligned), desc_host, workspace (256-byte aligned), "
+                                              "out and offsets (8-byte aligned) are required");
+    uint64_t filt = 0, segs = 0, bound = 0;
+    uint32_t max_h = 0;
+    for (uint32_t i = 0; i < n; ++i) {
+        const ssdnerf_png_bgr_desc& d = desc_host[i];
+        if (!bgr_dims_ok(d.h, d.w)) return set_error_msg(SSDNERF_ERR_ARG, "png_encode_bgr: an image size the layout refuses");
+        const PngGeom g = png_geom_rgb(1, d.h, d.w);
+        filt += g.raw; segs += g.nseg; bound += kFileOverhead + g.raw + 5ull * g.nseg;
+        max_h = std::max(max_h, d.h);
+    }
+    const uint64_t need = align256(filt) + align256(segs * kSlotBytes) + align256(segs * 4);
+    if (workspace_bytes < need || out_bytes < bound)
+        return set_error_msg(SSDNERF_ERR_ARG, "png_encode_bgr: workspace or out smaller than ssdnerf_png_bgr_layout's sizes");
+    static DeviceOnce once;
+    if (once.first())
+        SSDNERF_CUDA_OK(cudaFuncSetAttribute(k_png_deflate, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DeflateSmem)));
+    uint8_t* ws = static_cast<uint8_t*>(workspace);
+    uint8_t* slots = ws + align256(filt);
+    uint32_t* seg_info = reinterpret_cast<uint32_t*>(slots + align256(segs * kSlotBytes));
+    cudaStream_t s = (cudaStream_t)stream;
+    k_png_filter_bgr<<<dim3(div_up(max_h, 8), n), 256, 0, s>>>(images, desc, ws);
+    SSDNERF_LAUNCH_OK();
+    // one deflate grid per size: the layout put each size's filtered streams and segments next to each other
+    const std::vector<uint32_t> ord = bgr_order(desc_host, n);
+    for (uint32_t a = 0; a < n;) {
+        const ssdnerf_png_bgr_desc& d = desc_host[ord[a]];
+        uint32_t b = a + 1;
+        while (b < n && desc_host[ord[b]].h == d.h && desc_host[ord[b]].w == d.w) ++b;
+        const PngGeom g = png_geom_rgb(b - a, d.h, d.w);
+        for (uint32_t k = a; k < b; ++k) {
+            const ssdnerf_png_bgr_desc& e = desc_host[ord[k]];
+            if (e.filt_offset != d.filt_offset + (k - a) * g.raw || e.seg_first != d.seg_first + (k - a) * g.nseg ||
+                e.filt_offset + g.raw > filt || e.seg_first + g.nseg > segs)
+                return set_error_msg(SSDNERF_ERR_ARG, "png_encode_bgr: the descriptors are not laid out by ssdnerf_png_bgr_layout");
+        }
+        k_png_deflate<<<(b - a) * g.nseg, kDfThreads, sizeof(DeflateSmem), s>>>(g, ws + d.filt_offset, slots + (uint64_t)d.seg_first * kSlotBytes,
+                                                                             seg_info + d.seg_first);
+        SSDNERF_LAUNCH_OK();
+        a = b;
+    }
+    k_png_sizes_bgr<<<1, 1024, 0, s>>>(desc, n, seg_info, offsets);
+    SSDNERF_LAUNCH_OK();
+    k_png_write_bgr<<<n, kWriteThreads, 0, s>>>(desc, ws, slots, seg_info, offsets, out);
+    SSDNERF_LAUNCH_OK();
+    return 0;
+}
 
 extern "C" size_t ssdnerf_png_workspace_bytes(uint32_t n, uint32_t h, uint32_t w) {
     if (!png_dims_ok(n, h, w)) return 0;

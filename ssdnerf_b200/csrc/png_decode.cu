@@ -1,5 +1,6 @@
 // PNG decoding of dataset views on the device (C ABI section 9, include/ssdnerf_b200.h): the images the reference reads with
-// mmcv.imread(path, channel_order='rgb') -> cv2.imread(IMREAD_COLOR) in shapenet_srn.py, as float32 RGB / 255.
+// mmcv.imread(path, channel_order='rgb') -> cv2.imread(IMREAD_COLOR) in shapenet_srn.py, as float32 RGB / 255.  The raw decode (section
+// 10) reads KITTI's frames and instance maps as cv2.imread(IMREAD_UNCHANGED) does: 8-bit grey / BGR bytes or native-endian uint16.
 //
 // * k_png_decode: one warp per image.  Lane 0 runs the inflater (zlib header, stored / fixed / dynamic blocks, canonical Huffman
 //   tables with a first-level lookup in the warp's shared memory), writing literals itself; each match is broadcast and copied by the
@@ -390,7 +391,92 @@ __host__ __device__ inline bool desc_ok(const ssdnerf_png_desc& d, size_t stream
     return true;
 }
 
-// ------------------------------------------------------------------------------------------------ kernel
+// ------------------------------------------------------------------------------------------------ kernels
+// inflates, checks and unfilters one image with the calling warp; put(r, x, raw) takes each raw pixel (bytes packed little-endian)
+// as its row step completes.  Returns the image's status.  This is k_png_decode's body; k_png_decode keeps its own copy so that its
+// code stays as it was compiled before the raw decode existed.
+template <class Put>
+__device__ __forceinline__ int decode_warp(const uint8_t* stream, uint32_t stream_bytes, uint8_t* buf, uint32_t cap, uint32_t h, uint32_t w,
+                                           int bpp, InflateTables* tabs, int lane, Put put) {
+    // inflate: lane 0 decodes, the warp copies matches
+    Inflater inf;
+    int st = SSDNERF_PNG_OK;
+    uint32_t adler_want = 0;
+    if (lane == 0) {
+        inf.init(stream, stream_bytes, buf, cap, tabs);
+        if (!inf.header()) st = inf.status;
+    }
+    st = __shfl_sync(0xffffffffu, st, 0);
+    if (st == SSDNERF_PNG_OK) {
+        for (;;) {
+            int tok = kTokError;
+            uint32_t mlen = 0, mdist = 0, end = 0;
+            if (lane == 0) { tok = inf.next(mlen, mdist); end = inf.out; }
+            tok = __shfl_sync(0xffffffffu, tok, 0);
+            if (tok != kTokMatch) break;
+            mlen = __shfl_sync(0xffffffffu, mlen, 0);
+            mdist = __shfl_sync(0xffffffffu, mdist, 0);
+            end = __shfl_sync(0xffffffffu, end, 0);
+            __syncwarp();
+            const uint32_t o = end - mlen;
+            for (uint32_t p = lane; p < mlen; p += 32) buf[o + p] = buf[o - mdist + (p % mdist)];
+            __syncwarp();
+        }
+        if (lane == 0) {
+            if (inf.status == SSDNERF_PNG_OK) inf.trailer(adler_want);
+            st = inf.status;
+        }
+        st = __shfl_sync(0xffffffffu, st, 0);
+        adler_want = __shfl_sync(0xffffffffu, adler_want, 0);
+    }
+    __syncwarp();
+    if (st == SSDNERF_PNG_OK) {
+        uint64_t sa, sb;
+        adler_partial(buf, cap, lane, 32, sa, sb);
+        for (int o = 16; o; o >>= 1) {
+            sa += __shfl_xor_sync(0xffffffffu, sa, o);
+            sb += __shfl_xor_sync(0xffffffffu, sb, o);
+        }
+        if (adler_combine(cap, sa, sb) != adler_want) st = SSDNERF_PNG_BAD_ADLER;
+    }
+
+    // unfilter in place, row by row
+    const uint32_t stride = 1 + w * bpp;
+    for (uint32_t r = 0; r < h && st == SSDNERF_PNG_OK; ++r) {
+        uint8_t* row = buf + (size_t)r * stride;
+        const uint8_t* prior = r ? row - stride : nullptr;
+        const int f = row[0];
+        if (f > 4) { st = SSDNERF_PNG_BAD_FILTER; break; }
+        uint32_t carry = 0, carry_up = 0;
+        for (uint32_t x0 = 0; x0 < w; x0 += 32) {
+            const uint32_t x = x0 + lane, cnt = min(32u, w - x0);
+            const bool valid = lane < cnt;
+            const uint32_t fx = valid ? load_pixel(row + 1 + x * bpp, bpp) : 0;
+            const uint32_t up = valid && prior ? load_pixel(prior + 1 + x * bpp, bpp) : 0;
+            uint32_t upleft = __shfl_up_sync(0xffffffffu, up, 1);
+            if (lane == 0) upleft = carry_up;
+            uint32_t raw = 0;
+            if (f == 0 || f == 2) {
+                raw = unfilter_pixel(f, fx, 0, up, 0, bpp);
+            } else {
+                for (uint32_t s = 0; s < cnt; ++s) {
+                    uint32_t left = __shfl_sync(0xffffffffu, raw, (s + 31) & 31);
+                    if (s == 0) left = carry;
+                    if (lane == s) raw = unfilter_pixel(f, fx, left, up, upleft, bpp);
+                }
+            }
+            carry = __shfl_sync(0xffffffffu, raw, cnt - 1);
+            carry_up = __shfl_sync(0xffffffffu, up, cnt - 1);
+            if (valid) {
+                store_pixel(row + 1 + x * bpp, raw, bpp);
+                put(r, x, raw);
+            }
+        }
+        __syncwarp();
+    }
+    return st;
+}
+
 __global__ void __launch_bounds__(32 * kDecWarps, 8) k_png_decode(const uint8_t* __restrict__ streams, size_t stream_bytes,
                                                                   const ssdnerf_png_desc* __restrict__ descs, uint32_t n,
                                                                   uint8_t* __restrict__ work, size_t work_bytes, float* __restrict__ out,
@@ -493,10 +579,57 @@ __global__ void __launch_bounds__(32 * kDecWarps, 8) k_png_decode(const uint8_t*
     if (lane == 0) status[img] = st;
 }
 
+// bytes per pixel of the raw decode's formats: 8-bit grey or RGB, 16-bit grey (0 otherwise)
+__host__ __device__ inline int png_raw_bpp(int color_type, int bit_depth) {
+    if (bit_depth == 8) return color_type == 0 ? 1 : color_type == 2 ? 3 : 0;
+    return bit_depth == 16 && color_type == 0 ? 2 : 0;
+}
+// raw pixel -> cv2.IMREAD_UNCHANGED samples: the pixel's bytes reversed, which turns RGB into BGR and a big-endian 16-bit sample into
+// a little-endian one (grey8 is unchanged)
+__host__ __device__ inline void store_unchanged(uint8_t* o, uint32_t raw, int bpp) {
+    for (int c = 0; c < bpp; ++c) o[c] = (uint8_t)(raw >> (8 * (bpp - 1 - c)));
+}
+
+__host__ __device__ inline bool raw_desc_ok(const ssdnerf_png_raw_desc& d, size_t stream_bytes, size_t work_bytes, size_t out_bytes,
+                                            uint64_t& filtered) {
+    const int bpp = png_raw_bpp(d.color_type, d.bit_depth);
+    if (!bpp || d.h == 0 || d.w == 0) return false;
+    filtered = (uint64_t)d.h * (1 + (uint64_t)d.w * bpp);
+    if (filtered >= (1ull << 31)) return false;
+    if (d.stream_offset > stream_bytes || d.stream_bytes > stream_bytes - d.stream_offset) return false;
+    if (d.work_offset > work_bytes || filtered > work_bytes - d.work_offset) return false;
+    const uint64_t nb = (uint64_t)d.h * d.w * bpp;
+    if (d.out_offset > out_bytes || nb > out_bytes - d.out_offset) return false;
+    return true;
+}
+
+__global__ void __launch_bounds__(32 * kDecWarps, 8) k_png_decode_raw(const uint8_t* __restrict__ streams, size_t stream_bytes,
+                                                                      const ssdnerf_png_raw_desc* __restrict__ descs, uint32_t n,
+                                                                      uint8_t* __restrict__ work, size_t work_bytes,
+                                                                      uint8_t* __restrict__ out, size_t out_bytes,
+                                                                      int32_t* __restrict__ status) {
+    __shared__ InflateTables tabs[kDecWarps];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const uint32_t img = blockIdx.x * kDecWarps + wid;
+    if (img >= n) return;
+    const ssdnerf_png_raw_desc d = descs[img];
+    uint64_t filtered = 0;
+    if (!raw_desc_ok(d, stream_bytes, work_bytes, out_bytes, filtered)) {
+        if (lane == 0) status[img] = SSDNERF_PNG_BAD_DESC;
+        return;
+    }
+    const int bpp = png_raw_bpp(d.color_type, d.bit_depth);
+    uint8_t* dst = out + d.out_offset;
+    const int st = decode_warp(streams + d.stream_offset, d.stream_bytes, work + d.work_offset, (uint32_t)filtered, d.h, d.w, bpp,
+                               &tabs[wid], lane, [&](uint32_t r, uint32_t x, uint32_t raw) {
+                                   store_unchanged(dst + ((size_t)r * d.w + x) * bpp, raw, bpp);
+                               });
+    if (lane == 0) status[img] = st;
+}
+
 // the same decode, serially on the host
-static int png_decode_serial(const uint8_t* stream, uint32_t stream_bytes, uint32_t h, uint32_t w, int color_type, const uint8_t* palette,
-                             uint8_t* buf, float* out) {
-    const int bpp = png_bpp(color_type);
+template <class Put>
+static int decode_serial(const uint8_t* stream, uint32_t stream_bytes, uint32_t h, uint32_t w, int bpp, uint8_t* buf, Put put) {
     const uint32_t stride = 1 + w * bpp, cap = h * stride;
     InflateTables tabs;
     Inflater inf;
@@ -525,10 +658,7 @@ static int png_decode_serial(const uint8_t* stream, uint32_t stream_bytes, uint3
             const uint32_t up = prior ? load_pixel(prior + 1 + x * bpp, bpp) : 0;
             const uint32_t raw = unfilter_pixel(f, load_pixel(row + 1 + x * bpp, bpp), left, up, upleft, bpp);
             store_pixel(row + 1 + x * bpp, raw, bpp);
-            uint32_t rgb[3];
-            pixel_rgb(raw, color_type, palette, rgb);
-            float* o = out + ((size_t)r * w + x) * 3;
-            o[0] = div255(rgb[0]); o[1] = div255(rgb[1]); o[2] = div255(rgb[2]);
+            put(r, x, raw);
             left = raw; upleft = up;
         }
     }
@@ -566,6 +696,45 @@ extern "C" int ssdnerf_png_decode_host(const uint8_t* stream_host, size_t stream
     const size_t ws = ssdnerf_png_decode_workspace_bytes(h, w, color_type);
     if (!ws || stream_bytes > 0xFFFFFFFFu) return set_error_msg(SSDNERF_ERR_ARG, "png_decode_host: unsupported size or colour type");
     std::vector<uint8_t> buf(ws);
-    *status_host = png_decode_serial(stream_host, (uint32_t)stream_bytes, h, w, color_type, palette_host, buf.data(), out_host);
+    *status_host = decode_serial(stream_host, (uint32_t)stream_bytes, h, w, png_bpp(color_type), buf.data(), [&](uint32_t r, uint32_t x, uint32_t raw) {
+        uint32_t rgb[3];
+        pixel_rgb(raw, color_type, palette_host, rgb);
+        float* o = out_host + ((size_t)r * w + x) * 3;
+        o[0] = div255(rgb[0]); o[1] = div255(rgb[1]); o[2] = div255(rgb[2]);
+    });
+    return SSDNERF_OK;
+}
+
+extern "C" size_t ssdnerf_png_decode_raw_workspace_bytes(uint32_t h, uint32_t w, int color_type, int bit_depth) {
+    const int bpp = png_raw_bpp(color_type, bit_depth);
+    if (!bpp || h == 0 || w == 0) return 0;
+    const uint64_t filtered = (uint64_t)h * (1 + (uint64_t)w * bpp);
+    if (filtered >= (1ull << 31)) return 0;
+    return (size_t)((filtered + 15) & ~15ull);
+}
+
+extern "C" int ssdnerf_png_decode_raw(const uint8_t* streams, size_t stream_bytes, const ssdnerf_png_raw_desc* desc, uint32_t n,
+                                      void* workspace, size_t workspace_bytes, uint8_t* out, size_t out_bytes, int32_t* status, void* stream) {
+    if (n == 0) return SSDNERF_OK;
+    if (!streams || !desc || !workspace || !out || !status || ((uintptr_t)desc & 7u) || ((uintptr_t)status & 3u))
+        return set_error_msg(SSDNERF_ERR_ARG, "png_decode_raw: streams, desc, workspace, out and status must be (aligned) device pointers");
+    k_png_decode_raw<<<div_up(n, kDecWarps), 32 * kDecWarps, 0, (cudaStream_t)stream>>>(
+        streams, stream_bytes, desc, n, (uint8_t*)workspace, workspace_bytes, out, out_bytes, status);
+    SSDNERF_LAUNCH_OK();
+    return SSDNERF_OK;
+}
+
+extern "C" int ssdnerf_png_decode_raw_host(const uint8_t* stream_host, size_t stream_bytes, uint32_t h, uint32_t w, int color_type,
+                                           int bit_depth, uint8_t* out_host, int32_t* status_host) {
+    if (!status_host || !out_host || (!stream_host && stream_bytes))
+        return set_error_msg(SSDNERF_ERR_ARG, "png_decode_raw_host: stream_host, out_host and status_host are required");
+    const size_t ws = ssdnerf_png_decode_raw_workspace_bytes(h, w, color_type, bit_depth);
+    if (!ws || stream_bytes > 0xFFFFFFFFu)
+        return set_error_msg(SSDNERF_ERR_ARG, "png_decode_raw_host: unsupported size, colour type or bit depth");
+    const int bpp = png_raw_bpp(color_type, bit_depth);
+    std::vector<uint8_t> buf(ws);
+    *status_host = decode_serial(stream_host, (uint32_t)stream_bytes, h, w, bpp, buf.data(), [&](uint32_t r, uint32_t x, uint32_t raw) {
+        store_unchanged(out_host + ((size_t)r * w + x) * bpp, raw, bpp);
+    });
     return SSDNERF_OK;
 }
