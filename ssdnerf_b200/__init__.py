@@ -7,14 +7,16 @@
     mesh                : marching cubes + binary STL of save_mesh  (csrc/mesh.cu)
     viz                 : PNG files under viz_dir, interpolation demo (csrc/png.cu)
     datasets            : ShapeNet SRN scenes, GPU PNG decoding of their views (csrc/png_decode.cu)
+    evaluation          : the evaluation loop of tools/test.py (`evaluate_3d`, `SceneBatches`); `python -m ssdnerf_b200.test` runs it
 
 Everything computes through libssdnerf_b200.so (C ABI: include/ssdnerf_b200.h); there is no CPU or PyTorch fallback.
 """
 from .registry import DATASETS, MODELS, MODULES, build_dataset, build_model, build_module  # noqa: F401
 from .config import Config  # noqa: F401
-from . import activation, datasets, decoders, density, diffusion, mesh, nerf, raymarching, renderer, scene_cache, shencoder, unet, viz  # noqa: F401
+from . import activation, datasets, decoders, density, diffusion, evaluation, mesh, nerf, raymarching, renderer, scene_cache, shencoder, unet, viz  # noqa: F401
 from .datasets import ShapeNetSRN, collate, decode_png  # noqa: F401
 from .decoders import TriPlaneDecoder  # noqa: F401
+from .evaluation import SceneBatches, evaluate_3d  # noqa: F401
 from .diffusion import GaussianDiffusion  # noqa: F401
 from .nerf import DiffusionNeRF, MultiSceneNeRF  # noqa: F401
 from .unet import DenoisingUnetMod  # noqa: F401

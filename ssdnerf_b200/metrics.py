@@ -142,8 +142,8 @@ class FIDKID:
             self.fake_feats.append(feat); self.num_fake_feeded += feat.shape[0]
         return feat.shape[0]
 
-    @torch.no_grad()
-    def summary(self, generator=None):
+    def _fid(self):
+        """(first `num_images` fake features, fid, mean term, cov term); real statistics from the fed reals unless `prepare` loaded them"""
         if self.real_feats_all is None:
             feats = torch.cat(self.real_feats, dim=0)
             assert feats.shape[0] >= self.num_images
@@ -154,8 +154,30 @@ class FIDKID:
         fake = fake[:self.num_images]
         dev = fake.device
         fmean, fcov = feature_statistics(fake)
-        fid, mean, cov = frechet_distance(fmean, fcov, self.real_mean.to(dev), self.real_cov.to(dev))
-        kid = kernel_inception_distance(self.real_feats_all.to(dev), fake, self.num_subsets, self.max_subset_size, generator) * 1000
+        return (fake,) + frechet_distance(fmean, fcov, self.real_mean.to(dev), self.real_cov.to(dev))
+
+    @torch.no_grad()
+    def summary(self, generator=None):
+        fake, fid, mean, cov = self._fid()
+        kid = kernel_inception_distance(self.real_feats_all.to(fake.device), fake, self.num_subsets, self.max_subset_size, generator) * 1000
         self._result_dict = dict(fid=fid, fid_mean=mean, fid_cov=cov, kid=kid)
         self._result_str = f'{fid:.4f} ({mean:.5f}/{cov:.5f}), {kid:.4f}'
         return fid, mean, cov, kid
+
+
+@METRICS.register_module()
+class FID(FIDKID):
+    """mmgen's `FID` [mmgen-memory], the metric 17 of the 24 shipped configs name: FIDKID's features and Frechet distance without KID.
+    `bgr2rgb` defaults to True there (every shipped config sets it to False)."""
+    name = 'FID'
+
+    def __init__(self, num_images, image_shape=None, inception_pkl=None, bgr2rgb=True, inception_args=None, feature_fn=None):
+        super().__init__(num_images, feature_fn=feature_fn, inception_pkl=inception_pkl, inception_args=inception_args, bgr2rgb=bgr2rgb,
+                         image_shape=image_shape)
+
+    @torch.no_grad()
+    def summary(self):
+        _, fid, mean, cov = self._fid()
+        self._result_dict = dict(fid=fid, fid_mean=mean, fid_cov=cov)
+        self._result_str = f'{fid:.4f} ({mean:.5f}/{cov:.5f})'
+        return fid, mean, cov

@@ -4,17 +4,30 @@ Scenes are independent units (noise -> DDIM -> occupancy grid -> render): rank r
 reference's `DistributedSampler(shuffle=False)` (lib/datasets/samplers/distributed_sampler.py:53-59, `indices[rank::world]`).
 There is no collective on the data path; `gather_scene_outputs` is the eval-side exchange (the reference all-gathers Inception
 features inside mmgen's FID.feed; we gather whatever per-scene tensor the caller produced) and works with NCCL or gloo."""
+import math
+
 import torch
 import torch.distributed as dist
 
 
-def scene_indices(num_scenes, rank=None, world_size=None):
-    """indices of the scenes this rank processes (strided; ragged tails allowed)"""
+def scene_indices(num_scenes, rank=None, world_size=None, samples_per_gpu=None):
+    """indices of the scenes this rank processes (strided; ragged tails allowed).
+
+    With `samples_per_gpu`, the test loader's order under a distributed launch: mmgen's `DistributedSampler(shuffle=False)`
+    [mmgen-memory] gives every rank `ceil(N / W / samples_per_gpu) * samples_per_gpu` indices of the list 0..N-1 padded by repeating
+    its head, `indices[rank::W]`, so every rank runs the same number of full batches."""
     if rank is None:
         rank = dist.get_rank() if dist.is_available() and dist.is_initialized() else 0
     if world_size is None:
         world_size = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
-    return list(range(rank, num_scenes, world_size))
+    if samples_per_gpu is None:
+        return list(range(rank, num_scenes, world_size))
+    total = int(math.ceil(num_scenes * 1.0 / world_size / samples_per_gpu)) * samples_per_gpu * world_size
+    indices = list(range(num_scenes))
+    indices += indices[:total - num_scenes]
+    if len(indices) != total:        # the padding repeats the head once: the sampler's own assertion
+        raise ValueError(f'{num_scenes} scenes cannot fill {world_size} ranks x {total // world_size} samples')
+    return indices[rank::world_size]
 
 
 def gather_scene_outputs(local, num_scenes, group=None):
