@@ -612,6 +612,23 @@ SSDNERF_API int ssdnerf_png_encode_bgr(const uint8_t* images, const ssdnerf_png_
                                        uint32_t n, void* workspace, size_t workspace_bytes, uint8_t* out, size_t out_bytes,
                                        unsigned long long* offsets, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * 11. Exponential moving average of model state (csrc/ema.cu): mmgen's ExponentialMovingAverageHook with interp_mode='lerp'.
+ *    Every tensor of the state is updated by one launch (a table that overflows one kernel parameter block takes more), with no
+ *    allocation and no host-to-device copy, so the call can be captured in a CUDA graph.
+ * ------------------------------------------------------------------------------------------------ */
+typedef struct {
+    float* ema;               /* the moving average, updated in place */
+    const float* src;         /* the trained tensor it follows */
+    uint64_t n;               /* elements of both */
+    uint32_t trainable;       /* nonzero: the source is a parameter that requires grad (takes `momentum`) */
+} ssdnerf_ema_tensor;
+/* for each of the `count` tensors of the host table tensors_host: ema[i] = src[i] + (ema[i] - src[i]) * m, each operation rounded
+ * separately (no contraction), m = momentum for trainable entries and momentum_nontrainable otherwise; bit-identical to torch's
+ * `a + (b - a) * m` on fp32, NaN and inf included.  NULL pointers or a non-finite momentum are SSDNERF_ERR_ARG; count 0 is a no-op. */
+SSDNERF_API int ssdnerf_ema_lerp_f32(const ssdnerf_ema_tensor* tensors_host, uint32_t count, float momentum, float momentum_nontrainable,
+                                     void* stream);
+
 #ifdef __cplusplus
 }
 #endif

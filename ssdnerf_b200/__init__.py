@@ -8,12 +8,14 @@
     viz                 : PNG files under viz_dir, interpolation demo (csrc/png.cu)
     datasets            : ShapeNet SRN scenes, GPU PNG decoding of their views (csrc/png_decode.cu)
     evaluation          : the evaluation loop of tools/test.py (`evaluate_3d`, `SceneBatches`); `python -m ssdnerf_b200.test` runs it
+    runner / ema        : the training runner of tools/train.py and its hooks, the fused EMA update (csrc/ema.cu);
+                          `python -m ssdnerf_b200.train` runs it
 
 Everything computes through libssdnerf_b200.so (C ABI: include/ssdnerf_b200.h); there is no CPU or PyTorch fallback.
 """
 from .registry import DATASETS, MODELS, MODULES, build_dataset, build_model, build_module  # noqa: F401
 from .config import Config  # noqa: F401
-from . import activation, datasets, decoders, density, diffusion, evaluation, mesh, nerf, raymarching, renderer, scene_cache, shencoder, unet, viz  # noqa: F401
+from . import activation, datasets, decoders, density, diffusion, ema, evaluation, mesh, nerf, raymarching, renderer, runner, scene_cache, shencoder, unet, viz  # noqa: F401
 from .datasets import ShapeNetSRN, collate, decode_png  # noqa: F401
 from .decoders import TriPlaneDecoder  # noqa: F401
 from .evaluation import SceneBatches, evaluate_3d  # noqa: F401

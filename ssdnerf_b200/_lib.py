@@ -58,6 +58,11 @@ class RenderTrainArgs(ctypes.Structure):
     ]
 
 
+class EmaTensor(ctypes.Structure):
+    """mirror of `ssdnerf_ema_tensor` (include/ssdnerf_b200.h)"""
+    _fields_ = [('ema', c_void_p), ('src', c_void_p), ('n', ctypes.c_uint64), ('trainable', c_u32)]
+
+
 def lib():
     """Load the native library; raises if it has not been built (python -m ssdnerf_b200.build)."""
     global _lib
@@ -103,6 +108,8 @@ def lib():
         L.ssdnerf_kitti_resize_host.argtypes = [c_void_p, c_u32, c_u32, c_u32, c_u32, c_void_p]
         L.ssdnerf_png_bgr_layout.argtypes = [c_void_p, c_u32, c_void_p, c_void_p]
         L.ssdnerf_png_encode_bgr.argtypes = [c_void_p, c_void_p, c_void_p, c_u32, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p, c_void_p]
+        # exponential moving average (header section 11)
+        L.ssdnerf_ema_lerp_f32.argtypes = [ctypes.POINTER(EmaTensor), c_u32, c_f32, c_f32, c_void_p]
         _lib = L
     return _lib
 

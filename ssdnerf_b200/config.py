@@ -24,6 +24,16 @@ def _wrap(x):
     return x
 
 
+def _plain(x):
+    if isinstance(x, dict):
+        return {k: _plain(v) for k, v in x.items()}
+    if isinstance(x, (list, tuple)):
+        return type(x)(_plain(v) for v in x)
+    if isinstance(x, range):
+        return list(x)
+    return x
+
+
 def _merge(base, new):
     out = dict(base)
     for k, v in new.items():
@@ -55,6 +65,14 @@ class Config:
             return _C.fromfile(filename)
         except ImportError:
             return _wrap(_load(os.path.abspath(filename)))
+
+    @staticmethod
+    def dump(cfg, filename):
+        """writes `cfg` as a python config file, one `name = value` line per top-level key, that `fromfile` reads back to an equal
+        dict (values must be plain python literals: dicts, lists, tuples, strings, numbers, booleans, None)"""
+        with open(filename, 'w') as f:
+            for k, v in cfg.items():
+                f.write(f'{k} = {_plain(v)!r}\n')
 
     @staticmethod
     def merge_options(cfg, options):

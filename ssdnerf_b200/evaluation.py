@@ -29,13 +29,15 @@ class SceneBatches:
 
     One process takes every scene in order, the last batch partial.  In a distributed run (the default process group is initialised)
     each rank takes `sharding.scene_indices(len(dataset), rank, world, samples_per_gpu)`: the sampler's padded strided share, in full
-    batches.  With `prefetch`, one background thread reads the next batch's items (`dataset[i]`: the scenes' file bytes) while the
+    batches.  An explicit `indices` list (the training loader's order) replaces both.  With `prefetch`, one background thread reads the next batch's items (`dataset[i]`: the scenes' file bytes) while the
     caller runs the current one; `collate` (the PNG decode on the device) stays on the caller's thread and current stream, in order."""
 
-    def __init__(self, dataset, samples_per_gpu, device=None, prefetch=True):
+    def __init__(self, dataset, samples_per_gpu, device=None, prefetch=True, indices=None):
         self.dataset, self.samples_per_gpu, self.device, self.prefetch = dataset, samples_per_gpu, device, prefetch
         rank, world = _dist_info()
-        if dist.is_available() and dist.is_initialized():
+        if indices is not None:
+            self.indices = list(indices)
+        elif dist.is_available() and dist.is_initialized():
             self.indices = scene_indices(len(dataset), rank, world, samples_per_gpu)
         else:
             self.indices = list(range(len(dataset)))

@@ -149,8 +149,16 @@ def rgetattr(obj, attr, *default):
 
 
 def rsetattr(obj, attr, val):
+    """dotted setattr (lib/core/utils/misc.py:137-142); a name whose owner is a dict is set as an item, so plain-dict configs
+    (`train_cfg.optimizer.lr`) take settings as mmcv's ConfigDict does"""
     head, _, tail = attr.rpartition('.')
-    setattr(rgetattr(obj, head) if head else obj, tail, val)
+    owner = obj
+    for name in head.split('.') if head else []:
+        owner = owner[name] if isinstance(owner, dict) else getattr(owner, name)
+    if isinstance(owner, dict):
+        owner[tail] = val
+    else:
+        setattr(owner, tail, val)
 
 
 @contextmanager

@@ -5,7 +5,9 @@ reference's `DistributedSampler(shuffle=False)` (lib/datasets/samplers/distribut
 There is no collective on the data path; `gather_scene_outputs` is the eval-side exchange (the reference all-gathers Inception
 features inside mmgen's FID.feed; we gather whatever per-scene tensor the caller produced) and works with NCCL or gloo."""
 import math
+import random
 
+import numpy as np
 import torch
 import torch.distributed as dist
 
@@ -28,6 +30,53 @@ def scene_indices(num_scenes, rank=None, world_size=None, samples_per_gpu=None):
     if len(indices) != total:        # the padding repeats the head once: the sampler's own assertion
         raise ValueError(f'{num_scenes} scenes cannot fill {world_size} ranks x {total // world_size} samples')
     return indices[rank::world_size]
+
+
+def train_indices(num_scenes, epoch=0, seed=0, rank=0, world_size=1, samples_per_gpu=1, split_data=False, skip_iter=0):
+    """The scene order one rank trains on in epoch `epoch` under a distributed launch: the reference's `DistributedSampler`
+    (lib/datasets/samplers/distributed_sampler.py) with `shuffle=True`.  Without `split_data` (or on one rank) the whole list is
+    permuted by a `torch.Generator` seeded `seed + epoch`, padded by repeating its head to `ceil(N / W / spg) * spg * W` and strided
+    `[rank::W]`.  With `split_data` each rank permutes its own contiguous range `round(linspace(0, N, W + 1))` -- the scenes whose
+    latents `SceneCache` keeps on that rank -- padded to the longest range's batches.  The first `skip_iter` indices are dropped (a
+    resumed run's position in the epoch)."""
+    if split_data and world_size > 1:
+        points = np.round(np.linspace(0, num_scenes, num=world_size + 1)).astype(np.int64)
+        ranges = [torch.arange(start=int(points[r]), end=int(points[r + 1])) for r in range(world_size)]
+        num_samples = int(np.max([np.ceil(len(r) * 1.0 / samples_per_gpu) for r in ranges])) * samples_per_gpu
+        g = torch.Generator()
+        g.manual_seed(seed + epoch)
+        inds = ranges[rank]
+        indices = inds[torch.randperm(len(inds), generator=g)].tolist()
+        indices += indices[:(num_samples - len(indices))]
+    else:
+        num_samples = int(math.ceil(num_scenes * 1.0 / world_size / samples_per_gpu)) * samples_per_gpu
+        total = num_samples * world_size
+        g = torch.Generator()
+        g.manual_seed(seed + epoch)
+        indices = torch.randperm(num_scenes, generator=g).tolist()
+        indices += indices[:(total - len(indices))]
+        if len(indices) != total:
+            raise ValueError(f'{num_scenes} scenes cannot fill {world_size} ranks x {num_samples} samples')
+        indices = indices[rank:total:world_size]
+    return indices[skip_iter:]
+
+
+def disjoint_first_batch(indices, samples_per_gpu, last_batch, rng=random):
+    """The reference's `check_batch_disjoint` (lib/datasets/samplers/distributed_sampler.py:71-81) on one epoch's order, so that no
+    scene is read in the first batch of an epoch while its latent from the previous epoch's last batch may still be being written:
+    raises when the epoch's last two batches share a scene; when its first batch shares a scene with `last_batch` (the previous
+    epoch's last batch), the first batch is redrawn by `rng.choices` (python's global generator, as the reference) from the scenes
+    past the first two batches that are not in `last_batch`.  Returns (the order, the set of this epoch's last batch)."""
+    spg = samples_per_gpu
+    indices = list(indices)
+    if not set(indices[-2 * spg:-spg]).isdisjoint(indices[-spg:]):
+        raise RuntimeError('Batch Disjoint Check Failed! Dataset is too small.')
+    if not set(indices[:spg]).isdisjoint(last_batch):
+        pool = set(indices[2 * spg:]).difference(last_batch)
+        if len(pool) < spg:
+            raise RuntimeError('Batch Disjoint Check Failed! Dataset is too small.')
+        indices[:spg] = rng.choices(list(pool), k=spg)
+    return indices, set(indices[-spg:])
 
 
 def gather_scene_outputs(local, num_scenes, group=None):
