@@ -629,6 +629,37 @@ typedef struct {
 SSDNERF_API int ssdnerf_ema_lerp_f32(const ssdnerf_ema_tensor* tensors_host, uint32_t count, float momentum, float momentum_nontrainable,
                                      void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * 12. Baseline JPEG files of video frames (csrc/jpeg.cu).
+ *     replaces: the CPU encoder behind the GUI's "Export video" (lib/core/ssdnerf_gui.py, videoio / ffmpeg) and
+ *               np.round(image * 255).astype(np.uint8) of its frames.
+ *     n frames of one size h x w, RGB channels-last [n][h][w][3], become n JFIF files byte-identical to
+ *     cv2.imencode('.jpg', bgr, [IMWRITE_JPEG_QUALITY, quality]) with libjpeg-turbo's defaults: JFIF 1.01 (density 1:1, no
+ *     thumbnail), 4:2:0 (Y 2 x 2, Cb / Cr 1 x 1, ids 1 / 2 / 3), the T.81 Annex K tables (quantisation scaled by the quality as
+ *     libjpeg scales it, clamped to [1, 255]; standard Huffman tables), no restart markers; markers SOI APP0 DQT DQT SOF0 DHT x 4 SOS
+ *     ... EOI.  The arithmetic is integer throughout (oracle/jpeg_port.py states it).  A file's bytes depend only on its pixels and
+ *     the quality.  Output: file i is out[offsets[i] : offsets[i + 1]], offsets uint64 [n + 1] on the device (offsets[n] = total).
+ *     Bad arguments (n = 0, h or w outside [1, 65535], quality outside [1, 100], NULL or misaligned pointers, a workspace or output
+ *     smaller than the queries below) are SSDNERF_ERR_ARG before anything is launched.
+ * ---------------------------------------------------------------------------------------------- */
+/* the most Huffman-coded bits one 8 x 8 block can take: a DC code of at most 11 bits plus 11 appended bits (|DC difference| <= 2040),
+ * then at most 63 AC symbols (each nonzero coefficient one, each ZRL covering 16 zero coefficients, EOB only after a zero), each a
+ * code of at most 16 bits plus at most 10 appended bits: 22 + 63 x 26 */
+#define SSDNERF_JPEG_BLOCK_MAX_BITS 1660
+/* bytes of workspace (256-byte aligned) for n frames of h x w; 0 for invalid sizes (0, above 65535, or n ceil(h/16) ceil(w/16) >= 2^31) */
+SSDNERF_API size_t ssdnerf_jpeg_workspace_bytes(uint32_t n, uint32_t h, uint32_t w);
+/* the largest total the n files can take: n (623 header bytes + 2 EOI + 2 x 1245 M), M = ceil(h / 16) ceil(w / 16) MCUs of six
+ * blocks: 6 SSDNERF_JPEG_BLOCK_MAX_BITS / 8 = 1245 bytes of entropy-coded data per MCU, doubled for a 0x00 stuffed after every byte
+ * (the 1-bit padding of the last byte fits in the MCU's whole bytes); 0 for invalid sizes */
+SSDNERF_API size_t ssdnerf_jpeg_output_bound(uint32_t n, uint32_t h, uint32_t w);
+/* rgb u8 [n][h][w][3] device pointer */
+SSDNERF_API int ssdnerf_jpeg_encode_u8(const uint8_t* rgb, uint32_t n, uint32_t h, uint32_t w, int quality, void* workspace,
+                                       size_t workspace_bytes, uint8_t* out, size_t out_bytes, unsigned long long* offsets, void* stream);
+/* rgb fp32 [n][h][w][3] (4-byte aligned), each sample rint(x * 255) in fp32 (half to even), clamped to [0, 255] (NaN -> 0): over the
+ * renderer's output range this is np.round(x * 255).astype(np.uint8); nothing is stored as u8 in between */
+SSDNERF_API int ssdnerf_jpeg_encode_f32(const float* rgb, uint32_t n, uint32_t h, uint32_t w, int quality, void* workspace,
+                                        size_t workspace_bytes, uint8_t* out, size_t out_bytes, unsigned long long* offsets, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

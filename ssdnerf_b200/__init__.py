@@ -10,12 +10,14 @@
     evaluation          : the evaluation loop of tools/test.py (`evaluate_3d`, `SceneBatches`); `python -m ssdnerf_b200.test` runs it
     runner / ema        : the training runner of tools/train.py and its hooks, the fused EMA update (csrc/ema.cu);
                           `python -m ssdnerf_b200.train` runs it
+    video / orbit       : orbit videos of the GUI's export: baseline JPEG frames on the device (csrc/jpeg.cu) in a Motion-JPEG AVI;
+                          `python -m ssdnerf_b200.orbit` renders them
 
 Everything computes through libssdnerf_b200.so (C ABI: include/ssdnerf_b200.h); there is no CPU or PyTorch fallback.
 """
 from .registry import DATASETS, MODELS, MODULES, build_dataset, build_model, build_module  # noqa: F401
 from .config import Config  # noqa: F401
-from . import activation, datasets, decoders, density, diffusion, ema, evaluation, mesh, nerf, raymarching, renderer, runner, scene_cache, shencoder, unet, viz  # noqa: F401
+from . import activation, datasets, decoders, density, diffusion, ema, evaluation, mesh, nerf, raymarching, renderer, runner, scene_cache, shencoder, unet, video, viz  # noqa: F401
 from .datasets import ShapeNetSRN, collate, decode_png  # noqa: F401
 from .decoders import TriPlaneDecoder  # noqa: F401
 from .evaluation import SceneBatches, evaluate_3d  # noqa: F401

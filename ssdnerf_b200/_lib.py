@@ -110,6 +110,12 @@ def lib():
         L.ssdnerf_png_encode_bgr.argtypes = [c_void_p, c_void_p, c_void_p, c_u32, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p, c_void_p]
         # exponential moving average (header section 11)
         L.ssdnerf_ema_lerp_f32.argtypes = [ctypes.POINTER(EmaTensor), c_u32, c_f32, c_f32, c_void_p]
+        # JPEG encoding (header section 12)
+        for name in ('ssdnerf_jpeg_workspace_bytes', 'ssdnerf_jpeg_output_bound'):
+            getattr(L, name).argtypes = [c_u32, c_u32, c_u32]
+            getattr(L, name).restype = c_size_t
+        for name in ('ssdnerf_jpeg_encode_u8', 'ssdnerf_jpeg_encode_f32'):
+            getattr(L, name).argtypes = [c_void_p, c_u32, c_u32, c_u32, c_int, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p, c_void_p]
         _lib = L
     return _lib
 
