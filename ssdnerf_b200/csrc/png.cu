@@ -1,9 +1,10 @@
 // PNG encoding of evaluation images on the device (C ABI section 8, include/ssdnerf_b200.h): the image files the reference writes
 // with plt.imsave under `viz_dir` (base_nerf.py:574-608, triplane_decoder.py:186-194).  Only the compressed bytes leave the GPU.
 //
-// * k_png_filter (one warp per row): builds the row's 8-bit RGBA pixels from the float sources (view or colormap prologue, nothing
-//   stored as u8 in between), picks among None / Sub / Up / Average / Paeth the filter with the least sum of |signed bytes| (libpng's
-//   heuristic, ties to the lower type) and writes the filtered row into the image's filtered stream.
+// * k_png_filter (one warp per row): builds the row's pixels from its pixel source, picks among None / Sub / Up / Average / Paeth the
+//   filter with the least sum of |signed bytes| (libpng's heuristic, ties to the lower type) and writes the filtered row into the
+//   image's filtered stream.  PngSrc gives 8-bit RGBA from the float views or maps (view or colormap prologue, nothing stored as u8
+//   in between), BgrSrc 8-bit RGB from u8 BGR bytes.
 // * k_png_deflate (one CTA per segment): an image's filtered stream is cut into segments of whole rows (<= kSegCap bytes).  A segment
 //   is one deflate block that may reference the 32 KB before it: the window and the segment sit in shared memory.  Match finding is
 //   per position over a few candidates (the latest equal 3-byte hash before the chunk, the nearest equal hash in the warp,
@@ -14,10 +15,10 @@
 //   bytes.  A segment whose dynamic block would be larger than its stored form is marked stored.
 // * k_png_sizes / k_png_write: file sizes and offsets (one scan), then per file the signature, IHDR, one IDAT (zlib header, the
 //   segments, runs of stored segments re-cut into stored blocks of up to 65535 bytes, Adler-32 of the filtered stream) with its
-//   CRC-32 from per-thread partials combined by GF(2) shifts, and IEND.
-// * BGR u8 images of their own sizes (header section 10, KITTI crops): k_png_filter_bgr builds 8-bit RGB rows (colour type 2) from
-//   the bytes; images of one size lie next to each other in the workspace, so k_png_deflate runs unchanged once per size;
-//   k_png_sizes_bgr / k_png_write_bgr are the per-file versions of the two last passes.
+//   CRC-32 from per-thread partials combined by GF(2) shifts, and IEND.  A file layout gives each file's geometry, filtered stream,
+//   first segment and colour type: UniformFiles for a batch of one size (RGBA), BgrFiles for the BGR descriptors (RGB).
+// * BGR u8 images of their own sizes (header section 10, KITTI crops): images of one size lie next to each other in the workspace,
+//   so k_png_deflate runs once per size.
 // * Determinism: a file's bytes depend only on its pixels.  The only atomics are an integer max into the hash table, integer
 //   frequency counts and ORs into disjoint bit fields, whose results do not depend on their order.
 #include "common.cuh"
@@ -84,14 +85,15 @@ static const uint8_t kViridisHost[256][3] = SSDNERF_VIRIDIS_RGB;
 // ------------------------------------------------------------------------------------------------ geometry
 struct PngGeom {
     uint32_t n, h, w;
-    uint32_t rowbytes;        // 4 w + 1 (filter byte)
+    uint32_t rowbytes;        // bpp w + 1 (filter byte)
     uint64_t raw;             // filtered bytes per image
     uint32_t rps, nseg;       // rows per segment, segments per image
 };
-static PngGeom png_geom(uint32_t n, uint32_t h, uint32_t w) {
+// n images of h x w at bpp bytes per pixel
+__host__ __device__ inline PngGeom png_geom(uint32_t n, uint32_t h, uint32_t w, uint32_t bpp) {
     PngGeom g;
     g.n = n; g.h = h; g.w = w;
-    g.rowbytes = 4 * w + 1;
+    g.rowbytes = bpp * w + 1;
     g.raw = (uint64_t)h * g.rowbytes;
     g.rps = g.rowbytes <= (uint32_t)kSegCap ? kSegCap / g.rowbytes : 0;
     g.nseg = g.rps ? div_up(h, g.rps) : 0;
@@ -102,14 +104,31 @@ __device__ __forceinline__ uint32_t seg_len(const PngGeom& g, uint32_t s) {
     return (min(g.h, (s + 1) * g.rps) - s * g.rps) * g.rowbytes;
 }
 
-// ------------------------------------------------------------------------------------------------ pixel prologue
+// ------------------------------------------------------------------------------------------------ pixel sources
+// A filter source has kBpp bytes per pixel.  row(filt, r) places the calling warp on one row of one image (false when the warp has
+// no row): r.y, the width r.w and r.out, where the row's filter type and filtered bytes go.  pixel(r, y, x) is the packed pixel
+// (first byte in the low bits) of row y of r's image.
+
+// views and maps (header section 8): g.n images of one size, their rows in order along the grid; RGBA from the float prologue
 struct PngSrc {
+    static constexpr uint32_t kBpp = 4;
     int colormap;             // 0: view (pred [| real]), 1: 2-D map through viridis
     const float* pred;        // view: [n][h][wv][3]
     const float* real;        // view, optional: [n][h][wv][3], left of pred
     uint32_t wv;
     const float* map;         // colormap: [n][h][w]
     float vmin, vrange;
+    PngGeom g;
+
+    struct Row { uint32_t img, y, w; uint8_t* out; };
+    __device__ __forceinline__ bool row(uint8_t* filt, Row& r) const {
+        const uint32_t i = blockIdx.x * 8 + (threadIdx.x >> 5);
+        if (i >= g.n * g.h) return false;
+        r.img = i / g.h; r.y = i % g.h; r.w = g.w;
+        r.out = filt + r.img * g.raw + (uint64_t)r.y * g.rowbytes;
+        return true;
+    }
+    __device__ __forceinline__ uint32_t pixel(const Row& r, uint32_t y, uint32_t x) const;
 };
 
 // base_nerf.py:551-553 then 580-581: round(clamp(x, 0, 1) * 255) / 255, then round(. * 255) to uint8 (both round half to even)
@@ -122,7 +141,8 @@ __device__ __forceinline__ uint32_t pred_byte(float x) {
 __device__ __forceinline__ uint32_t real_byte(float x) { return (uint32_t)(int)__fmul_rn(x, 255.0f) & 0xFFu; }
 
 // packed RGBA (R in the low byte) of pixel (y, x) of image i
-__device__ __forceinline__ uint32_t png_pixel(const PngSrc& s, const PngGeom& g, uint32_t i, uint32_t y, uint32_t x) {
+__device__ __forceinline__ uint32_t png_pixel(const PngSrc& s, uint32_t i, uint32_t y, uint32_t x) {
+    const PngGeom& g = s.g;
     if (!s.colormap) {
         const float* src = s.pred;
         uint32_t xs = x;
@@ -148,6 +168,28 @@ __device__ __forceinline__ uint32_t png_pixel(const PngSrc& s, const PngGeom& g,
     }
     return (uint32_t)kViridis[idx][0] | ((uint32_t)kViridis[idx][1] << 8) | ((uint32_t)kViridis[idx][2] << 16) | 0xFF000000u;
 }
+__device__ __forceinline__ uint32_t PngSrc::pixel(const Row& r, uint32_t y, uint32_t x) const { return png_pixel(*this, r.img, y, x); }
+
+// u8 BGR images of their own sizes (header section 10): one grid column of rows / 8 CTAs per image; RGB
+struct BgrSrc {
+    static constexpr uint32_t kBpp = 3;
+    const uint8_t* images;
+    const ssdnerf_png_bgr_desc* desc;
+
+    struct Row { const uint8_t* src; uint32_t y, w; uint8_t* out; };
+    __device__ __forceinline__ bool row(uint8_t* ws, Row& r) const {
+        const ssdnerf_png_bgr_desc d = desc[blockIdx.y];
+        r.y = blockIdx.x * 8 + (threadIdx.x >> 5);
+        if (r.y >= d.h) return false;
+        r.src = images + d.src_offset; r.w = d.w;
+        r.out = ws + d.filt_offset + (uint64_t)r.y * (kBpp * d.w + 1);
+        return true;
+    }
+    __device__ __forceinline__ uint32_t pixel(const Row& r, uint32_t y, uint32_t x) const {
+        const uint8_t* p = r.src + ((uint64_t)y * r.w + x) * 3;
+        return (uint32_t)p[2] | ((uint32_t)p[1] << 8) | ((uint32_t)p[0] << 16);
+    }
+};
 
 __device__ __forceinline__ int paeth(int a, int b, int c) {
     const int p = a + b - c, pa = abs(p - a), pb = abs(p - b), pc = abs(p - c);
@@ -160,30 +202,33 @@ __device__ __forceinline__ uint32_t filt_byte(int t, int x, int a, int b, int c)
 }
 
 // ------------------------------------------------------------------------------------------------ filter pass: one warp per row
-__global__ void __launch_bounds__(256) k_png_filter(PngSrc s, PngGeom g, uint8_t* __restrict__ filt) {
-    const uint32_t row = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-    if (row >= g.n * g.h) return;
-    const uint32_t img = row / g.h, y = row % g.h;
-    uint8_t* out = filt + img * g.raw + (uint64_t)y * g.rowbytes;
+template <class Src>
+__global__ void __launch_bounds__(256) k_png_filter(Src s, uint8_t* __restrict__ filt) {
+    constexpr uint32_t bpp = Src::kBpp;
+    const uint32_t lane = threadIdx.x & 31;
+    typename Src::Row r;
+    if (!s.row(filt, r)) return;
+    const uint32_t y = r.y, w = r.w;
+    uint8_t* out = r.out;
     uint32_t best = 0;
     for (int pass = 0; pass < 2; ++pass) {
         uint32_t sum[5] = {0, 0, 0, 0, 0};
         uint32_t carry_cur = 0, carry_up = 0;
-        for (uint32_t x0 = 0; x0 < g.w; x0 += 32) {
+        for (uint32_t x0 = 0; x0 < w; x0 += 32) {
             const uint32_t x = x0 + lane;
             uint32_t cur = 0, up = 0;
-            if (x < g.w) {
-                cur = png_pixel(s, g, img, y, x);
-                up = y ? png_pixel(s, g, img, y - 1, x) : 0u;
+            if (x < w) {
+                cur = s.pixel(r, y, x);
+                up = y ? s.pixel(r, y - 1, x) : 0u;
             }
             uint32_t left = __shfl_up_sync(0xffffffffu, cur, 1), ul = __shfl_up_sync(0xffffffffu, up, 1);
             if (lane == 0) { left = carry_cur; ul = carry_up; }
             carry_cur = __shfl_sync(0xffffffffu, cur, 31);
             carry_up = __shfl_sync(0xffffffffu, up, 31);
-            if (x < g.w) {
+            if (x < w) {
                 if (pass == 0) {
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) {
+                    for (int k = 0; k < (int)bpp; ++k) {
                         const int xv = (cur >> (8 * k)) & 0xFF, a = (left >> (8 * k)) & 0xFF, b = (up >> (8 * k)) & 0xFF,
                                   c = (ul >> (8 * k)) & 0xFF;
 #pragma unroll
@@ -191,9 +236,9 @@ __global__ void __launch_bounds__(256) k_png_filter(PngSrc s, PngGeom g, uint8_t
                     }
                 } else {
 #pragma unroll
-                    for (int k = 0; k < 4; ++k)
-                        out[1 + 4 * x + k] = (uint8_t)filt_byte((int)best, (cur >> (8 * k)) & 0xFF, (left >> (8 * k)) & 0xFF,
-                                                                (up >> (8 * k)) & 0xFF, (ul >> (8 * k)) & 0xFF);
+                    for (int k = 0; k < (int)bpp; ++k)
+                        out[1 + bpp * x + k] = (uint8_t)filt_byte((int)best, (cur >> (8 * k)) & 0xFF, (left >> (8 * k)) & 0xFF,
+                                                                  (up >> (8 * k)) & 0xFF, (ul >> (8 * k)) & 0xFF);
                 }
             }
         }
@@ -579,11 +624,33 @@ __global__ void __launch_bounds__(kDfThreads, 1) k_png_deflate(PngGeom g, const 
 }
 
 // ------------------------------------------------------------------------------------------------ file sizes, offsets, assembly
+// A file layout gives file f's geometry, the offset of its filtered stream and the index of its first segment (file(f)), and the
+// IHDR colour type of its files (kColorType).
+struct PngFile {
+    PngGeom g;
+    uint64_t filt, seg;
+};
+// views and maps: g.n files of one size, one after the other
+struct UniformFiles {
+    static constexpr uint8_t kColorType = 6;                  // 8-bit RGBA
+    PngGeom g;
+    __device__ __forceinline__ PngFile file(uint32_t f) const { return {g, f * g.raw, (uint64_t)f * g.nseg}; }
+};
+// BGR images: the descriptors' own sizes and places (ssdnerf_png_bgr_layout)
+struct BgrFiles {
+    static constexpr uint8_t kColorType = 2;                  // 8-bit RGB
+    const ssdnerf_png_bgr_desc* desc;
+    __device__ __forceinline__ PngFile file(uint32_t f) const {
+        const ssdnerf_png_bgr_desc d = desc[f];
+        return {png_geom(1, d.h, d.w, BgrSrc::kBpp), d.filt_offset, d.seg_first};
+    }
+};
+
 __device__ __forceinline__ uint64_t stored_run_bytes(uint64_t R) { return R + 5 * ((R + 65534) / 65535); }
 
-__device__ uint64_t deflate_bytes(const PngGeom& g, const uint32_t* seg_info, uint32_t img) {
-    const uint32_t* info = seg_info + (uint64_t)img * g.nseg;
-    uint64_t total = 0;
+// bytes of a file whose segments' sizes are info[0, g.nseg)
+__device__ uint64_t file_bytes(const PngGeom& g, const uint32_t* info) {
+    uint64_t total = kFileOverhead;
     for (uint32_t s = 0; s < g.nseg;) {
         if (info[s] != kStored) { total += info[s++]; continue; }
         uint64_t R = 0;
@@ -594,11 +661,14 @@ __device__ uint64_t deflate_bytes(const PngGeom& g, const uint32_t* seg_info, ui
 }
 
 // offsets[i] = first byte of file i, offsets[n] = total (one CTA)
-__global__ void __launch_bounds__(1024) k_png_sizes(PngGeom g, const uint32_t* __restrict__ seg_info, unsigned long long* offsets) {
+template <class Files>
+__global__ void __launch_bounds__(1024) k_png_sizes(Files files, uint32_t n, const uint32_t* __restrict__ seg_info,
+                                                    unsigned long long* offsets) {
     __shared__ uint64_t wsum[32];
-    const uint32_t tid = threadIdx.x, per = div_up(g.n, 1024), f0 = min(tid * per, g.n), f1 = min(f0 + per, g.n);
+    const uint32_t tid = threadIdx.x, per = div_up(n, 1024), f0 = min(tid * per, n), f1 = min(f0 + per, n);
+    auto bytes = [&](uint32_t f) { const PngFile pf = files.file(f); return file_bytes(pf.g, seg_info + pf.seg); };
     uint64_t mine = 0;
-    for (uint32_t f = f0; f < f1; ++f) mine += kFileOverhead + deflate_bytes(g, seg_info, f);
+    for (uint32_t f = f0; f < f1; ++f) mine += bytes(f);
     uint64_t incl = mine;
     for (int o = 1; o < 32; o <<= 1) {
         const uint64_t t = __shfl_up_sync(0xffffffffu, incl, o);
@@ -609,25 +679,29 @@ __global__ void __launch_bounds__(1024) k_png_sizes(PngGeom g, const uint32_t* _
     uint64_t base = 0, total = 0;
     for (uint32_t k = 0; k < 32; ++k) { if (k < (tid >> 5)) base += wsum[k]; total += wsum[k]; }
     uint64_t o = base + incl - mine;
-    for (uint32_t f = f0; f < f1; ++f) { offsets[f] = o; o += kFileOverhead + deflate_bytes(g, seg_info, f); }
-    if (tid == 0) offsets[g.n] = total;
+    for (uint32_t f = f0; f < f1; ++f) { offsets[f] = o; o += bytes(f); }
+    if (tid == 0) offsets[n] = total;
 }
 
 __device__ __forceinline__ void put_be32(uint8_t* p, uint32_t v) {
     p[0] = (uint8_t)(v >> 24); p[1] = (uint8_t)(v >> 16); p[2] = (uint8_t)(v >> 8); p[3] = (uint8_t)v;
 }
 
-__global__ void __launch_bounds__(kWriteThreads) k_png_write(PngGeom g, const uint8_t* __restrict__ filt, const uint8_t* __restrict__ slots,
+// one CTA per file
+template <class Files>
+__global__ void __launch_bounds__(kWriteThreads) k_png_write(Files files, const uint8_t* __restrict__ filt, const uint8_t* __restrict__ slots,
                                                             const uint32_t* __restrict__ seg_info,
                                                             const unsigned long long* __restrict__ offsets, uint8_t* __restrict__ out) {
     __shared__ uint32_t tab[256];
     __shared__ uint32_t pcrc[kWriteThreads];
     __shared__ uint64_t plen[kWriteThreads], ps1[kWriteThreads], ps2[kWriteThreads];
     const uint32_t f = blockIdx.x, tid = threadIdx.x;
+    const PngFile pf = files.file(f);
+    const PngGeom& g = pf.g;
     tab[tid] = crc_table_entry(tid);
     uint8_t* o = out + offsets[f];
     const uint64_t dlen = offsets[f + 1] - offsets[f] - kFileOverhead;
-    const uint8_t* fraw = filt + f * g.raw;
+    const uint8_t* fraw = filt + pf.filt;
     __syncthreads();
     if (tid == 0) {
         const uint8_t sig[8] = {0x89, 'P', 'N', 'G', '\r', '\n', 0x1A, '\n'};
@@ -635,7 +709,7 @@ __global__ void __launch_bounds__(kWriteThreads) k_png_write(PngGeom g, const ui
         put_be32(o + 8, 13);
         o[12] = 'I'; o[13] = 'H'; o[14] = 'D'; o[15] = 'R';
         put_be32(o + 16, g.w); put_be32(o + 20, g.h);
-        o[24] = 8; o[25] = 6; o[26] = 0; o[27] = 0; o[28] = 0;      // 8-bit RGBA, deflate, adaptive filtering, no interlace
+        o[24] = 8; o[25] = Files::kColorType; o[26] = 0; o[27] = 0; o[28] = 0;   // 8-bit, deflate, adaptive filtering, no interlace
         uint32_t c = 0xFFFFFFFFu;
         for (int i = 12; i < 29; ++i) c = tab[(c ^ o[i]) & 0xFF] ^ (c >> 8);
         put_be32(o + 29, ~c);
@@ -644,11 +718,11 @@ __global__ void __launch_bounds__(kWriteThreads) k_png_write(PngGeom g, const ui
         o[41] = 0x78; o[42] = 0x9C;                                    // zlib: deflate, 32 KB window, check bits
     }
     // deflate stream: dynamic segments from their slots, runs of stored segments as stored blocks of <= 65535 bytes
-    const uint32_t* info = seg_info + (uint64_t)f * g.nseg;
+    const uint32_t* info = seg_info + pf.seg;
     uint64_t pos = 43;
     for (uint32_t s = 0; s < g.nseg;) {
         if (info[s] != kStored) {
-            const uint8_t* slot = slots + ((uint64_t)f * g.nseg + s) * kSlotBytes;
+            const uint8_t* slot = slots + (pf.seg + s) * kSlotBytes;
             for (uint32_t i = tid; i < info[s]; i += kWriteThreads) o[pos + i] = slot[i];
             pos += info[s++];
             continue;
@@ -704,17 +778,17 @@ __global__ void __launch_bounds__(kWriteThreads) k_png_write(PngGeom g, const ui
     }
 }
 
-static bool png_dims_ok(uint32_t n, uint32_t h, uint32_t w) {
+static bool png_dims_ok(uint32_t n, uint32_t h, uint32_t w, uint32_t bpp) {
     if (!n || !h || !w) return false;
-    const PngGeom g = png_geom(n, h, w);
+    const PngGeom g = png_geom(n, h, w, bpp);
     return g.rps && g.raw < (1ull << 31) && (uint64_t)n * g.nseg < (1ull << 31) && (uint64_t)n * h < (1ull << 31);
 }
 static uint64_t align256(uint64_t b) { return (b + 255) & ~(uint64_t)255; }
 
-static int png_encode(const PngSrc& src, uint32_t n, uint32_t h, uint32_t w, void* workspace, size_t workspace_bytes, uint8_t* out,
+static int png_encode(PngSrc src, uint32_t n, uint32_t h, uint32_t w, void* workspace, size_t workspace_bytes, uint8_t* out,
                       size_t out_bytes, unsigned long long* offsets, void* stream, const char* who) {
     static thread_local char msg[256];
-    if (!png_dims_ok(n, h, w)) {
+    if (!png_dims_ok(n, h, w, PngSrc::kBpp)) {
         snprintf(msg, sizeof(msg), "%s: n, h, w must be >= 1 and a row (4 w + 1 bytes) at most %d bytes (w <= %d), got n=%u h=%u w=%u",
                  who, kSegCap, (kSegCap - 1) / 4, n, h, w);
         return set_error_msg(SSDNERF_ERR_ARG, msg);
@@ -735,209 +809,25 @@ static int png_encode(const PngSrc& src, uint32_t n, uint32_t h, uint32_t w, voi
     static DeviceOnce once;
     if (once.first())
         SSDNERF_CUDA_OK(cudaFuncSetAttribute(k_png_deflate, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DeflateSmem)));
-    const PngGeom g = png_geom(n, h, w);
+    const PngGeom g = png_geom(n, h, w, PngSrc::kBpp);
+    src.g = g;
     const uint64_t nsegs = (uint64_t)n * g.nseg;
     uint8_t* filt = static_cast<uint8_t*>(workspace);
     uint8_t* slots = filt + align256((uint64_t)n * g.raw);
     uint32_t* seg_info = reinterpret_cast<uint32_t*>(slots + align256(nsegs * kSlotBytes));
     cudaStream_t s = (cudaStream_t)stream;
-    k_png_filter<<<div_up(n * h, 8), 256, 0, s>>>(src, g, filt);
+    k_png_filter<<<div_up(n * h, 8), 256, 0, s>>>(src, filt);
     SSDNERF_LAUNCH_OK();
     k_png_deflate<<<(uint32_t)nsegs, kDfThreads, sizeof(DeflateSmem), s>>>(g, filt, slots, seg_info);
     SSDNERF_LAUNCH_OK();
-    k_png_sizes<<<1, 1024, 0, s>>>(g, seg_info, offsets);
+    k_png_sizes<<<1, 1024, 0, s>>>(UniformFiles{g}, n, seg_info, offsets);
     SSDNERF_LAUNCH_OK();
-    k_png_write<<<n, kWriteThreads, 0, s>>>(g, filt, slots, seg_info, offsets, out);
+    k_png_write<<<n, kWriteThreads, 0, s>>>(UniformFiles{g}, filt, slots, seg_info, offsets, out);
     SSDNERF_LAUNCH_OK();
     return 0;
 }
 
 // ------------------------------------------------------------------------------------------------ BGR u8 images of their own sizes
-// one image's geometry at 3 bytes per pixel (the deflate and assembly of one size group read it like png_geom's)
-__host__ __device__ inline PngGeom png_geom_rgb(uint32_t n, uint32_t h, uint32_t w) {
-    PngGeom g;
-    g.n = n; g.h = h; g.w = w;
-    g.rowbytes = 3 * w + 1;
-    g.raw = (uint64_t)h * g.rowbytes;
-    g.rps = g.rowbytes <= (uint32_t)kSegCap ? kSegCap / g.rowbytes : 0;
-    g.nseg = g.rps ? (h + g.rps - 1) / g.rps : 0;
-    return g;
-}
-
-// one warp per row (grid: rows / 8 x images): the row's RGB bytes from BGR, the least-sum filter as k_png_filter picks it
-__global__ void __launch_bounds__(256) k_png_filter_bgr(const uint8_t* __restrict__ images, const ssdnerf_png_bgr_desc* __restrict__ desc,
-                                                        uint8_t* __restrict__ ws) {
-    const ssdnerf_png_bgr_desc d = desc[blockIdx.y];
-    const uint32_t y = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-    if (y >= d.h) return;
-    const uint32_t rowbytes = 3 * d.w + 1;
-    uint8_t* out = ws + d.filt_offset + (uint64_t)y * rowbytes;
-    const uint8_t* src = images + d.src_offset;
-    auto pix = [&](uint32_t yy, uint32_t x) {
-        const uint8_t* p = src + ((uint64_t)yy * d.w + x) * 3;
-        return (uint32_t)p[2] | ((uint32_t)p[1] << 8) | ((uint32_t)p[0] << 16);
-    };
-    uint32_t best = 0;
-    for (int pass = 0; pass < 2; ++pass) {
-        uint32_t sum[5] = {0, 0, 0, 0, 0};
-        uint32_t carry_cur = 0, carry_up = 0;
-        for (uint32_t x0 = 0; x0 < d.w; x0 += 32) {
-            const uint32_t x = x0 + lane;
-            uint32_t cur = 0, up = 0;
-            if (x < d.w) {
-                cur = pix(y, x);
-                up = y ? pix(y - 1, x) : 0u;
-            }
-            uint32_t left = __shfl_up_sync(0xffffffffu, cur, 1), ul = __shfl_up_sync(0xffffffffu, up, 1);
-            if (lane == 0) { left = carry_cur; ul = carry_up; }
-            carry_cur = __shfl_sync(0xffffffffu, cur, 31);
-            carry_up = __shfl_sync(0xffffffffu, up, 31);
-            if (x < d.w) {
-                if (pass == 0) {
-#pragma unroll
-                    for (int k = 0; k < 3; ++k) {
-                        const int xv = (cur >> (8 * k)) & 0xFF, a = (left >> (8 * k)) & 0xFF, b = (up >> (8 * k)) & 0xFF,
-                                  c = (ul >> (8 * k)) & 0xFF;
-#pragma unroll
-                        for (int t = 0; t < 5; ++t) sum[t] += abs((int)(int8_t)filt_byte(t, xv, a, b, c));
-                    }
-                } else {
-#pragma unroll
-                    for (int k = 0; k < 3; ++k)
-                        out[1 + 3 * x + k] = (uint8_t)filt_byte((int)best, (cur >> (8 * k)) & 0xFF, (left >> (8 * k)) & 0xFF,
-                                                                (up >> (8 * k)) & 0xFF, (ul >> (8 * k)) & 0xFF);
-                }
-            }
-        }
-        if (pass == 0) {
-#pragma unroll
-            for (int t = 0; t < 5; ++t)
-                for (int o = 16; o; o >>= 1) sum[t] += __shfl_xor_sync(0xffffffffu, sum[t], o);
-            for (int t = 1; t < 5; ++t)
-                if (sum[t] < sum[best]) best = t;
-            if (lane == 0) out[0] = (uint8_t)best;
-        }
-    }
-}
-
-__device__ __forceinline__ uint64_t bgr_file_bytes(const ssdnerf_png_bgr_desc& d, const uint32_t* seg_info) {
-    return kFileOverhead + deflate_bytes(png_geom_rgb(1, d.h, d.w), seg_info + d.seg_first, 0);
-}
-
-// offsets[i] = first byte of file i, offsets[n] = total (one CTA), as k_png_sizes
-__global__ void __launch_bounds__(1024) k_png_sizes_bgr(const ssdnerf_png_bgr_desc* __restrict__ desc, uint32_t n,
-                                                        const uint32_t* __restrict__ seg_info, unsigned long long* offsets) {
-    __shared__ uint64_t wsum[32];
-    const uint32_t tid = threadIdx.x, per = div_up(n, 1024), f0 = min(tid * per, n), f1 = min(f0 + per, n);
-    uint64_t mine = 0;
-    for (uint32_t f = f0; f < f1; ++f) mine += bgr_file_bytes(desc[f], seg_info);
-    uint64_t incl = mine;
-    for (int o = 1; o < 32; o <<= 1) {
-        const uint64_t t = __shfl_up_sync(0xffffffffu, incl, o);
-        if ((tid & 31) >= (uint32_t)o) incl += t;
-    }
-    if ((tid & 31) == 31) wsum[tid >> 5] = incl;
-    __syncthreads();
-    uint64_t base = 0, total = 0;
-    for (uint32_t k = 0; k < 32; ++k) { if (k < (tid >> 5)) base += wsum[k]; total += wsum[k]; }
-    uint64_t o = base + incl - mine;
-    for (uint32_t f = f0; f < f1; ++f) { offsets[f] = o; o += bgr_file_bytes(desc[f], seg_info); }
-    if (tid == 0) offsets[n] = total;
-}
-
-// one CTA per file, as k_png_write with the file's own geometry and colour type 2
-__global__ void __launch_bounds__(kWriteThreads) k_png_write_bgr(const ssdnerf_png_bgr_desc* __restrict__ desc, const uint8_t* __restrict__ ws,
-                                                                const uint8_t* __restrict__ slots, const uint32_t* __restrict__ seg_info,
-                                                                const unsigned long long* __restrict__ offsets, uint8_t* __restrict__ out) {
-    __shared__ uint32_t tab[256];
-    __shared__ uint32_t pcrc[kWriteThreads];
-    __shared__ uint64_t plen[kWriteThreads], ps1[kWriteThreads], ps2[kWriteThreads];
-    const uint32_t f = blockIdx.x, tid = threadIdx.x;
-    const ssdnerf_png_bgr_desc d = desc[f];
-    const PngGeom g = png_geom_rgb(1, d.h, d.w);
-    tab[tid] = crc_table_entry(tid);
-    uint8_t* o = out + offsets[f];
-    const uint64_t dlen = offsets[f + 1] - offsets[f] - kFileOverhead;
-    const uint8_t* fraw = ws + d.filt_offset;
-    __syncthreads();
-    if (tid == 0) {
-        const uint8_t sig[8] = {0x89, 'P', 'N', 'G', '\r', '\n', 0x1A, '\n'};
-        for (int i = 0; i < 8; ++i) o[i] = sig[i];
-        put_be32(o + 8, 13);
-        o[12] = 'I'; o[13] = 'H'; o[14] = 'D'; o[15] = 'R';
-        put_be32(o + 16, g.w); put_be32(o + 20, g.h);
-        o[24] = 8; o[25] = 2; o[26] = 0; o[27] = 0; o[28] = 0;      // 8-bit RGB, deflate, adaptive filtering, no interlace
-        uint32_t c = 0xFFFFFFFFu;
-        for (int i = 12; i < 29; ++i) c = tab[(c ^ o[i]) & 0xFF] ^ (c >> 8);
-        put_be32(o + 29, ~c);
-        put_be32(o + 33, (uint32_t)(dlen + 6));
-        o[37] = 'I'; o[38] = 'D'; o[39] = 'A'; o[40] = 'T';
-        o[41] = 0x78; o[42] = 0x9C;
-    }
-    const uint32_t* info = seg_info + d.seg_first;
-    uint64_t pos = 43;
-    for (uint32_t s = 0; s < g.nseg;) {
-        if (info[s] != kStored) {
-            const uint8_t* slot = slots + ((uint64_t)d.seg_first + s) * kSlotBytes;
-            for (uint32_t i = tid; i < info[s]; i += kWriteThreads) o[pos + i] = slot[i];
-            pos += info[s++];
-            continue;
-        }
-        const uint32_t s_first = s;
-        uint64_t R = 0;
-        while (s < g.nseg && info[s] == kStored) R += seg_len(g, s++);
-        const uint8_t* src = fraw + seg_start(g, s_first);
-        for (uint64_t done = 0; done < R;) {
-            const uint32_t L = (uint32_t)(R - done < 65535 ? R - done : 65535);
-            if (tid == 0) {
-                o[pos] = (s == g.nseg && done + L == R) ? 1 : 0;
-                o[pos + 1] = (uint8_t)L; o[pos + 2] = (uint8_t)(L >> 8);
-                o[pos + 3] = (uint8_t)~L; o[pos + 4] = (uint8_t)(~L >> 8);
-            }
-            for (uint32_t i = tid; i < L; i += kWriteThreads) o[pos + 5 + i] = src[done + i];
-            pos += 5 + L;
-            done += L;
-        }
-    }
-    {
-        uint64_t s1 = 0, s2 = 0;
-        for (uint64_t i = tid; i < g.raw; i += kWriteThreads) { const uint64_t b = fraw[i]; s1 += b; s2 += ((g.raw - i) % 65521) * b; }
-        ps1[tid] = s1 % 65521; ps2[tid] = s2 % 65521;
-        __syncthreads();
-        if (tid == 0) {
-            uint64_t a = 1, b = g.raw % 65521;
-            for (int k = 0; k < kWriteThreads; ++k) { a += ps1[k]; b += ps2[k]; }
-            put_be32(o + 43 + dlen, (uint32_t)((b % 65521) << 16 | (a % 65521)));
-        }
-    }
-    __syncthreads();
-    const uint64_t L = 4 + dlen + 6, chunk = (L + kWriteThreads - 1) / kWriteThreads;
-    const uint64_t a0 = min(L, tid * chunk), a1 = min(L, a0 + chunk);
-    uint32_t c = 0;
-    for (uint64_t i = a0; i < a1; ++i) c = tab[(c ^ o[37 + i]) & 0xFF] ^ (c >> 8);
-    pcrc[tid] = c; plen[tid] = a1 - a0;
-    __syncthreads();
-    for (uint32_t dd = 1; dd < kWriteThreads; dd <<= 1) {
-        if ((tid & (2 * dd - 1)) == 0 && plen[tid + dd]) {
-            pcrc[tid] = multmodp(crc_shift_op(plen[tid + dd]), pcrc[tid]) ^ pcrc[tid + dd];
-            plen[tid] += plen[tid + dd];
-        }
-        __syncthreads();
-    }
-    if (tid == 0) {
-        const uint32_t crc = ~(multmodp(crc_shift_op(L), 0xFFFFFFFFu) ^ pcrc[0]);
-        put_be32(o + 47 + dlen, crc);
-        const uint8_t iend[12] = {0, 0, 0, 0, 'I', 'E', 'N', 'D', 0xAE, 0x42, 0x60, 0x82};
-        for (int i = 0; i < 12; ++i) o[51 + dlen + i] = iend[i];
-    }
-}
-
-static bool bgr_dims_ok(uint32_t h, uint32_t w) {
-    if (!h || !w) return false;
-    const PngGeom g = png_geom_rgb(1, h, w);
-    return g.rps && g.raw < (1ull << 31);
-}
-
 // the images' order in the workspace: by size (h, then w), stable
 static std::vector<uint32_t> bgr_order(const ssdnerf_png_bgr_desc* d, uint32_t n) {
     std::vector<uint32_t> ord(n);
@@ -955,13 +845,13 @@ extern "C" int ssdnerf_png_bgr_layout(ssdnerf_png_bgr_desc* desc_host, uint32_t 
     uint64_t filt = 0, segs = 0, bound = 0;
     for (uint32_t i : bgr_order(desc_host, n)) {
         ssdnerf_png_bgr_desc& d = desc_host[i];
-        if (!bgr_dims_ok(d.h, d.w)) {
+        if (!png_dims_ok(1, d.h, d.w, BgrSrc::kBpp)) {
             static thread_local char msg[160];
             snprintf(msg, sizeof(msg), "png_bgr_layout: image %u is %u x %u; h, w >= 1 and a row (3 w + 1 bytes) at most %d bytes", i, d.h, d.w,
                      kSegCap);
             return set_error_msg(SSDNERF_ERR_ARG, msg);
         }
-        const PngGeom g = png_geom_rgb(1, d.h, d.w);
+        const PngGeom g = png_geom(1, d.h, d.w, BgrSrc::kBpp);
         d.filt_offset = filt;
         d.seg_first = (uint32_t)segs;
         filt += g.raw;
@@ -986,8 +876,8 @@ extern "C" int ssdnerf_png_encode_bgr(const uint8_t* images, const ssdnerf_png_b
     uint32_t max_h = 0;
     for (uint32_t i = 0; i < n; ++i) {
         const ssdnerf_png_bgr_desc& d = desc_host[i];
-        if (!bgr_dims_ok(d.h, d.w)) return set_error_msg(SSDNERF_ERR_ARG, "png_encode_bgr: an image size the layout refuses");
-        const PngGeom g = png_geom_rgb(1, d.h, d.w);
+        if (!png_dims_ok(1, d.h, d.w, BgrSrc::kBpp)) return set_error_msg(SSDNERF_ERR_ARG, "png_encode_bgr: an image size the layout refuses");
+        const PngGeom g = png_geom(1, d.h, d.w, BgrSrc::kBpp);
         filt += g.raw; segs += g.nseg; bound += kFileOverhead + g.raw + 5ull * g.nseg;
         max_h = std::max(max_h, d.h);
     }
@@ -1001,7 +891,7 @@ extern "C" int ssdnerf_png_encode_bgr(const uint8_t* images, const ssdnerf_png_b
     uint8_t* slots = ws + align256(filt);
     uint32_t* seg_info = reinterpret_cast<uint32_t*>(slots + align256(segs * kSlotBytes));
     cudaStream_t s = (cudaStream_t)stream;
-    k_png_filter_bgr<<<dim3(div_up(max_h, 8), n), 256, 0, s>>>(images, desc, ws);
+    k_png_filter<<<dim3(div_up(max_h, 8), n), 256, 0, s>>>(BgrSrc{images, desc}, ws);
     SSDNERF_LAUNCH_OK();
     // one deflate grid per size: the layout put each size's filtered streams and segments next to each other
     const std::vector<uint32_t> ord = bgr_order(desc_host, n);
@@ -1009,7 +899,7 @@ extern "C" int ssdnerf_png_encode_bgr(const uint8_t* images, const ssdnerf_png_b
         const ssdnerf_png_bgr_desc& d = desc_host[ord[a]];
         uint32_t b = a + 1;
         while (b < n && desc_host[ord[b]].h == d.h && desc_host[ord[b]].w == d.w) ++b;
-        const PngGeom g = png_geom_rgb(b - a, d.h, d.w);
+        const PngGeom g = png_geom(b - a, d.h, d.w, BgrSrc::kBpp);
         for (uint32_t k = a; k < b; ++k) {
             const ssdnerf_png_bgr_desc& e = desc_host[ord[k]];
             if (e.filt_offset != d.filt_offset + (k - a) * g.raw || e.seg_first != d.seg_first + (k - a) * g.nseg ||
@@ -1021,23 +911,23 @@ extern "C" int ssdnerf_png_encode_bgr(const uint8_t* images, const ssdnerf_png_b
         SSDNERF_LAUNCH_OK();
         a = b;
     }
-    k_png_sizes_bgr<<<1, 1024, 0, s>>>(desc, n, seg_info, offsets);
+    k_png_sizes<<<1, 1024, 0, s>>>(BgrFiles{desc}, n, seg_info, offsets);
     SSDNERF_LAUNCH_OK();
-    k_png_write_bgr<<<n, kWriteThreads, 0, s>>>(desc, ws, slots, seg_info, offsets, out);
+    k_png_write<<<n, kWriteThreads, 0, s>>>(BgrFiles{desc}, ws, slots, seg_info, offsets, out);
     SSDNERF_LAUNCH_OK();
     return 0;
 }
 
 extern "C" size_t ssdnerf_png_workspace_bytes(uint32_t n, uint32_t h, uint32_t w) {
-    if (!png_dims_ok(n, h, w)) return 0;
-    const PngGeom g = png_geom(n, h, w);
+    if (!png_dims_ok(n, h, w, PngSrc::kBpp)) return 0;
+    const PngGeom g = png_geom(n, h, w, PngSrc::kBpp);
     const uint64_t nsegs = (uint64_t)n * g.nseg;
     return align256((uint64_t)n * g.raw) + align256(nsegs * kSlotBytes) + align256(nsegs * 4);
 }
 
 extern "C" size_t ssdnerf_png_output_bound(uint32_t n, uint32_t h, uint32_t w) {
-    if (!png_dims_ok(n, h, w)) return 0;
-    const PngGeom g = png_geom(n, h, w);
+    if (!png_dims_ok(n, h, w, PngSrc::kBpp)) return 0;
+    const PngGeom g = png_geom(n, h, w, PngSrc::kBpp);
     return (size_t)n * (kFileOverhead + g.raw + 5ull * g.nseg);
 }
 

@@ -40,15 +40,13 @@ class PngInfo:
     __slots__ = ('name', 'w', 'h', 'color_type', 'palette', 'idat', 'stream_bytes')
 
 
-def parse_png(data, name='<bytes>'):
-    """Checks the signature and every chunk's CRC, parses IHDR / PLTE, gathers the IDAT payloads.  Raises ValueError naming the file
-    for a malformed file and NotImplementedError for what the decoder does not cover: bit depths other than 8, Adam7 interlacing,
-    and an eXIf chunk (cv2 would rotate the image by it)."""
+def png_chunks(data, name):
+    """Yields (type, body) for each chunk of a PNG file before IEND, with the checks every PNG reader here makes: the signature,
+    chunks inside the file, every chunk's CRC, IHDR first, once and 13 bytes long, and an IEND chunk.  Raises ValueError naming the
+    file."""
     mv = memoryview(data)
     if bytes(mv[:8]) != PNG_SIGNATURE:
         raise ValueError(f'{name}: not a PNG file (bad signature)')
-    info = PngInfo()
-    info.name, info.palette, info.idat = name, None, []
     pos, seen_ihdr = 8, False
     while True:
         if pos + 12 > len(mv):
@@ -65,8 +63,22 @@ def parse_png(data, name='<bytes>'):
         if ctype == b'IHDR':
             if seen_ihdr or length != 13:
                 raise ValueError(f'{name}: bad IHDR chunk')
-            w, h, depth, ct, comp, filt, interlace = struct.unpack('>IIBBBBB', body)
             seen_ihdr = True
+        elif ctype == b'IEND':
+            return
+        yield ctype, body
+        pos += 12 + length
+
+
+def parse_png(data, name='<bytes>'):
+    """Checks the file's chunks (png_chunks), parses IHDR / PLTE, gathers the IDAT payloads.  Raises ValueError naming the file
+    for a malformed file and NotImplementedError for what the decoder does not cover: bit depths other than 8, Adam7 interlacing,
+    and an eXIf chunk (cv2 would rotate the image by it)."""
+    info = PngInfo()
+    info.name, info.palette, info.idat = name, None, []
+    for ctype, body in png_chunks(data, name):
+        if ctype == b'IHDR':
+            w, h, depth, ct, comp, filt, interlace = struct.unpack('>IIBBBBB', body)
             if w == 0 or h == 0 or w >= 2 ** 31 or h >= 2 ** 31:
                 raise ValueError(f'{name}: IHDR size {w} x {h} is invalid')
             if ct not in _BPP:
@@ -79,16 +91,13 @@ def parse_png(data, name='<bytes>'):
                 raise ValueError(f'{name}: unknown compression or filter method in IHDR')
             info.w, info.h, info.color_type = w, h, ct
         elif ctype == b'PLTE':
-            if length % 3 or not 3 <= length <= 768:
+            if len(body) % 3 or not 3 <= len(body) <= 768:
                 raise ValueError(f'{name}: bad PLTE chunk')
-            info.palette = bytes(body) + bytes(768 - length)
+            info.palette = bytes(body) + bytes(768 - len(body))
         elif ctype == b'IDAT':
             info.idat.append(body)
         elif ctype == b'eXIf':
             raise NotImplementedError(f'{name}: eXIf chunk (cv2 would apply its orientation) is not supported')
-        elif ctype == b'IEND':
-            break
-        pos += 12 + length
     if not info.idat:
         raise ValueError(f'{name}: no IDAT chunk')
     if info.color_type == 3 and info.palette is None:

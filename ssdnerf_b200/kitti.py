@@ -13,14 +13,13 @@ import argparse
 import ctypes
 import os
 import struct
-import zlib
 from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import torch
 
 from . import _lib as N
-from .datasets import PNG_SIGNATURE, STATUS_REASONS
+from .datasets import STATUS_REASONS, png_chunks
 
 _RAW_DESC = np.dtype([('stream_offset', '<u8'), ('work_offset', '<u8'), ('out_offset', '<u8'), ('stream_bytes', '<u4'), ('h', '<u4'),
                       ('w', '<u4'), ('color_type', '<i4'), ('bit_depth', '<i4'), ('reserved', '<u4')])
@@ -112,30 +111,12 @@ def pose_text(c2w):
 # ------------------------------------------------------------------------------------------------ PNG chunks (8 and 16 bits)
 def parse_png_raw(data, name):
     """(h, w, colour type, bit depth, zlib stream) of a non-interlaced PNG; ValueError naming the file when malformed"""
-    mv = memoryview(data)
-    if bytes(mv[:8]) != PNG_SIGNATURE:
-        raise ValueError(f'{name}: not a PNG file (bad signature)')
-    pos, ihdr, idat = 8, None, []
-    while True:
-        if pos + 12 > len(mv):
-            raise ValueError(f'{name}: file ends before the IEND chunk')
-        length, ctype = struct.unpack('>I4s', mv[pos:pos + 8])
-        if length > len(mv) - pos - 12:
-            raise ValueError(f'{name}: chunk {ctype!r} runs past the end of the file')
-        body = mv[pos + 8:pos + 8 + length]
-        if zlib.crc32(body, zlib.crc32(ctype)) != struct.unpack('>I', mv[pos + 8 + length:pos + 12 + length])[0]:
-            raise ValueError(f'{name}: bad CRC in chunk {ctype!r}')
-        if ihdr is None and ctype != b'IHDR':
-            raise ValueError(f'{name}: the first chunk is {ctype!r}, not IHDR')
+    ihdr, idat = None, []
+    for ctype, body in png_chunks(data, name):
         if ctype == b'IHDR':
-            if ihdr is not None or length != 13:
-                raise ValueError(f'{name}: bad IHDR chunk')
             ihdr = struct.unpack('>IIBBBBB', body)
         elif ctype == b'IDAT':
             idat.append(bytes(body))
-        elif ctype == b'IEND':
-            break
-        pos += 12 + length
     w, h, depth, ct, comp, filt, interlace = ihdr
     if not idat or comp or filt or interlace or w == 0 or h == 0:
         raise ValueError(f'{name}: unsupported or malformed PNG header / data')
