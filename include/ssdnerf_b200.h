@@ -660,6 +660,47 @@ SSDNERF_API int ssdnerf_jpeg_encode_u8(const uint8_t* rgb, uint32_t n, uint32_t 
 SSDNERF_API int ssdnerf_jpeg_encode_f32(const float* rgb, uint32_t n, uint32_t h, uint32_t w, int quality, void* workspace,
                                         size_t workspace_bytes, uint8_t* out, size_t out_bytes, unsigned long long* offsets, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * 13. H.264 access units of video frames (csrc/h264.cu).
+ *     replaces: the libx264 encoder behind the GUI's "Export video" (lib/core/ssdnerf_gui.py, videoio.VideoWriter(lossless=False)).
+ *     n frames of one size h x w, RGB channels-last [n][h][w][3], become a Constrained Baseline H.264 stream (profile_idc 66 with
+ *     constraint_set0 / constraint_set1, 8-bit 4:2:0, CAVLC): every frame one IDR access unit of one I slice (idr_pic_id the parity
+ *     of first_frame + i for frame i, so batches of one video alternate it), every macroblock I_16x16 at the constant qp, modes by least SATD.  The SPS carries the smallest
+ *     level of Table A-1 whose MaxFS, frame-dimension and MaxMBPS limits hold at fps_num / fps_den (MaxBR is not enforced; 5.2 when no
+ *     level's MaxMBPS holds), the crop to h x w and a VUI of limited-range BT.601 (primaries, transfer, matrix 6).  The loop filter is
+ *     on (the decoder applies it).  oracle/h264_port.py states the integer rules.  An access unit's bytes depend only on its pixels,
+ *     qp and the parity of first_frame + i.
+ *     Output, offsets uint64 [n + 3] on the device: the SPS NAL unit is out[offsets[0] : offsets[1]], the PPS out[offsets[1] :
+ *     offsets[2]] (NAL units without start code or length, as an avcC record holds them), access unit i out[offsets[2 + i] :
+ *     offsets[3 + i]]: its IDR slice NAL unit behind a 4-byte big-endian length (an MP4 sample).
+ *     Bad arguments (n = 0, odd h or w, h or w < 2, more than level 5.2's 36864 macroblocks or 543 per side, qp outside
+ *     [SSDNERF_H264_MIN_QP, 51], fps_num or fps_den 0, NULL or misaligned pointers, a workspace or output smaller than the queries
+ *     below) are SSDNERF_ERR_ARG before anything is launched.
+ * ---------------------------------------------------------------------------------------------- */
+/* the smallest qp at which every level of 8-bit input fits Baseline's level_prefix <= 15 (|level| <= 2063): the Intra16x16 DC path
+ * bounds it, |Hadamard| <= 16 x 16 x 255 = 65280 gives (65280 MF(qp % 6, 0) + 4 f) >> (17 + qp / 6) = 2331 at qp 9 and 2040 at 10
+ * (the AC path reaches 583 and the chroma DC path 1166 at qp 9; the derivation is in oracle/h264_port.py) */
+#define SSDNERF_H264_MIN_QP 10
+/* the most CAVLC bits one macroblock can take: mb_type, chroma mode and mb_qp_delta 15; a 16-coefficient block at most
+ * 16 + 3 + 16 x 28 + 9 + 15 x 11 = 641, a 15-coefficient one 602, a chroma DC block 135: 15 + 641 + 24 x 602 + 2 x 135, rounded up to
+ * whole bytes */
+#define SSDNERF_H264_MB_MAX_BITS 15384
+/* bytes of workspace (256-byte aligned) for n frames of h x w; 0 for invalid sizes */
+SSDNERF_API size_t ssdnerf_h264_workspace_bytes(uint32_t n, uint32_t h, uint32_t w);
+/* the largest total the output can take: 2 x 64 bytes of SPS / PPS, then per frame a 5-byte length and NAL header plus R + R / 2 + 1
+ * bytes, R = 4 + M SSDNERF_H264_MB_MAX_BITS / 8 bytes of RBSP for M macroblocks (slice header and stop bit within the 4), with at
+ * most one emulation-prevention byte per two RBSP bytes; 0 for invalid sizes */
+SSDNERF_API size_t ssdnerf_h264_output_bound(uint32_t n, uint32_t h, uint32_t w);
+/* rgb u8 [n][h][w][3] device pointer */
+SSDNERF_API int ssdnerf_h264_encode_u8(const uint8_t* rgb, uint32_t n, uint32_t h, uint32_t w, int qp, uint32_t fps_num, uint32_t fps_den,
+                                       uint32_t first_frame, void* workspace, size_t workspace_bytes, uint8_t* out, size_t out_bytes, unsigned long long* offsets,
+                                       void* stream);
+/* rgb fp32 [n][h][w][3] (4-byte aligned), each sample rint(x * 255) in fp32, clamped to [0, 255] (NaN -> 0), as in
+ * ssdnerf_jpeg_encode_f32 */
+SSDNERF_API int ssdnerf_h264_encode_f32(const float* rgb, uint32_t n, uint32_t h, uint32_t w, int qp, uint32_t fps_num, uint32_t fps_den,
+                                        uint32_t first_frame, void* workspace, size_t workspace_bytes, uint8_t* out, size_t out_bytes, unsigned long long* offsets,
+                                        void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -10,8 +10,8 @@
     evaluation          : the evaluation loop of tools/test.py (`evaluate_3d`, `SceneBatches`); `python -m ssdnerf_b200.test` runs it
     runner / ema        : the training runner of tools/train.py and its hooks, the fused EMA update (csrc/ema.cu);
                           `python -m ssdnerf_b200.train` runs it
-    video / orbit       : orbit videos of the GUI's export: baseline JPEG frames on the device (csrc/jpeg.cu) in a Motion-JPEG AVI;
-                          `python -m ssdnerf_b200.orbit` renders them
+    video / orbit       : orbit videos of the GUI's export: baseline JPEG frames on the device (csrc/jpeg.cu) in a Motion-JPEG AVI,
+                          or all-intra H.264 (csrc/h264.cu) in an MP4; `python -m ssdnerf_b200.orbit` renders them
 
 Everything computes through libssdnerf_b200.so (C ABI: include/ssdnerf_b200.h); there is no CPU or PyTorch fallback.
 """

@@ -116,6 +116,13 @@ def lib():
             getattr(L, name).restype = c_size_t
         for name in ('ssdnerf_jpeg_encode_u8', 'ssdnerf_jpeg_encode_f32'):
             getattr(L, name).argtypes = [c_void_p, c_u32, c_u32, c_u32, c_int, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p, c_void_p]
+        # H.264 encoding (header section 13)
+        for name in ('ssdnerf_h264_workspace_bytes', 'ssdnerf_h264_output_bound'):
+            getattr(L, name).argtypes = [c_u32, c_u32, c_u32]
+            getattr(L, name).restype = c_size_t
+        for name in ('ssdnerf_h264_encode_u8', 'ssdnerf_h264_encode_f32'):
+            getattr(L, name).argtypes = [c_void_p, c_u32, c_u32, c_u32, c_int, c_u32, c_u32, c_u32, c_void_p, c_size_t, c_void_p, c_size_t,
+                                         c_void_p, c_void_p]
         _lib = L
     return _lib
 

@@ -8,14 +8,15 @@
 //   rounding quantisation and the zigzag; luma blocks wholly past the image edge are dummy blocks (zero AC, the DC of the block
 //   before them in the MCU).  Output int16 coefficients [MCU][6][64].
 // * k_jpeg_lengths (one thread per MCU): each block's DC difference from the previous block of its component in scan order and the
-//   Huffman-coded length of the MCU; k_jpeg_scan turns the lengths into bit offsets within the frame.
+//   Huffman-coded length of the MCU; k_frame_scan (bitstream.cuh) turns the lengths into bit offsets within the frame.
 // * k_jpeg_pack (one thread per MCU): the MCU's codes OR-ed into its disjoint bit field of the frame's zeroed stream (32-bit words,
 //   first bit in bit 31); the frame's last MCU pads the last byte with 1-bits.
-// * k_jpeg_ffcount / k_jpeg_scan / k_jpeg_offsets / k_jpeg_write: 0xFF bytes counted per 32-byte chunk and scanned, file sizes and
+// * k_jpeg_ffcount / k_frame_scan / k_file_offsets / k_jpeg_write: 0xFF bytes counted per 32-byte chunk and scanned, file sizes and
 //   offsets, then each chunk copied with a 0x00 stuffed after every 0xFF, behind the per-(h, w, quality) header built on the host,
 //   and EOI.
 // * Determinism: a file's bytes depend only on its pixels and the quality.  The only atomics are ORs into disjoint bit fields.
 #include "common.cuh"
+#include "bitstream.cuh"
 #include "../../include/ssdnerf_b200.h"
 #include <cstdio>
 #include <cstring>
@@ -360,36 +361,6 @@ __global__ void __launch_bounds__(256) k_jpeg_pack(const int16_t* __restrict__ c
 }
 
 // ------------------------------------------------------------------------------------------------ scans, stuffing, assembly
-// per frame (one CTA each): out[i] = sum of in[j < i] over the frame's `count` values, totals[f] = their sum
-__global__ void __launch_bounds__(1024) k_jpeg_scan(const uint32_t* __restrict__ in, uint64_t count, uint64_t* __restrict__ out,
-                                                    uint64_t* __restrict__ totals) {
-    __shared__ uint64_t wsum[32];
-    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const uint64_t base = (uint64_t)blockIdx.x * count;
-    uint64_t carry = 0;
-    for (uint64_t i0 = 0; i0 < count; i0 += 1024) {
-        const uint64_t i = i0 + tid;
-        const uint64_t v = i < count ? in[base + i] : 0;
-        uint64_t incl = v;
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint64_t t = __shfl_up_sync(0xffffffffu, incl, o);
-            if (lane >= (uint32_t)o) incl += t;
-        }
-        if (lane == 31) wsum[warp] = incl;
-        __syncthreads();
-        uint64_t before = 0, total = 0;
-        for (uint32_t k = 0; k < 32; ++k) {
-            const uint64_t s = wsum[k];
-            before += k < warp ? s : 0;
-            total += s;
-        }
-        if (i < count) out[base + i] = carry + before + incl - v;
-        carry += total;
-        __syncthreads();
-    }
-    if (tid == 0) totals[blockIdx.x] = carry;
-}
-
 __device__ __forceinline__ uint8_t stream_byte(const uint32_t* fw, uint64_t k) { return (uint8_t)(fw[k >> 2] >> (24 - 8 * (k & 3))); }
 
 // grid (chunks / 256, n): 0xFF bytes of each 32-byte chunk of the frame's stream (0 past its end)
@@ -414,35 +385,6 @@ __global__ void __launch_bounds__(256) k_jpeg_ffcount(const uint32_t* __restrict
         }
     }
     chunk_ff[(uint64_t)f * g.chunks + c] = cnt;
-}
-
-// one CTA: file f is header + stuffed stream + EOI; offsets[f] their exclusive sum, offsets[n] the total
-__global__ void __launch_bounds__(1024) k_jpeg_offsets(JpegGeom g, uint32_t header_len, const uint64_t* __restrict__ frame_bits,
-                                                       const uint64_t* __restrict__ frame_ff, unsigned long long* offsets) {
-    __shared__ uint64_t wsum[32];
-    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    uint64_t carry = 0;
-    for (uint32_t i0 = 0; i0 < g.n; i0 += 1024) {
-        const uint32_t i = i0 + tid;
-        const uint64_t v = i < g.n ? header_len + ((frame_bits[i] + 7) >> 3) + frame_ff[i] + 2 : 0;
-        uint64_t incl = v;
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint64_t t = __shfl_up_sync(0xffffffffu, incl, o);
-            if (lane >= (uint32_t)o) incl += t;
-        }
-        if (lane == 31) wsum[warp] = incl;
-        __syncthreads();
-        uint64_t before = 0, total = 0;
-        for (uint32_t k = 0; k < 32; ++k) {
-            const uint64_t s = wsum[k];
-            before += k < warp ? s : 0;
-            total += s;
-        }
-        if (i < g.n) offsets[i] = carry + before + incl - v;
-        carry += total;
-        __syncthreads();
-    }
-    if (tid == 0) offsets[g.n] = carry;
 }
 
 // grid (chunks / 256, n): each chunk's bytes with a 0x00 after every 0xFF; CTA x == 0 also writes the header and EOI
@@ -569,16 +511,16 @@ int jpeg_encode(const T* src, uint32_t n, uint32_t h, uint32_t w, int quality, v
     SSDNERF_LAUNCH_OK();
     k_jpeg_lengths<<<(uint32_t)((mcus + 255) / 256), 256, 0, st>>>(s.coef, g, ht, s.mcu_bits);
     SSDNERF_LAUNCH_OK();
-    k_jpeg_scan<<<n, 1024, 0, st>>>(s.mcu_bits, g.mpf, s.mcu_off, s.frame_bits);
+    k_frame_scan<<<n, 1024, 0, st>>>(s.mcu_bits, g.mpf, s.mcu_off, s.frame_bits);
     SSDNERF_LAUNCH_OK();
     SSDNERF_CUDA_OK(cudaMemsetAsync(s.words, 0, (uint64_t)n * g.words * 4, st));
     k_jpeg_pack<<<(uint32_t)((mcus + 255) / 256), 256, 0, st>>>(s.coef, g, ht, s.mcu_off, s.frame_bits, s.words);
     SSDNERF_LAUNCH_OK();
     k_jpeg_ffcount<<<chunk_grid, 256, 0, st>>>(s.words, g, s.frame_bits, s.chunk_ff);
     SSDNERF_LAUNCH_OK();
-    k_jpeg_scan<<<n, 1024, 0, st>>>(s.chunk_ff, g.chunks, s.chunk_off, s.frame_ff);
+    k_frame_scan<<<n, 1024, 0, st>>>(s.chunk_ff, g.chunks, s.chunk_off, s.frame_ff);
     SSDNERF_LAUNCH_OK();
-    k_jpeg_offsets<<<1, 1024, 0, st>>>(g, hdr.len, s.frame_bits, s.frame_ff, offsets);
+    k_file_offsets<<<1, 1024, 0, st>>>(n, 0, hdr.len + 2, s.frame_bits, s.frame_ff, offsets);
     SSDNERF_LAUNCH_OK();
     k_jpeg_write<<<chunk_grid, 256, 0, st>>>(s.words, g, hdr, s.frame_bits, s.chunk_off, offsets, out);
     SSDNERF_LAUNCH_OK();

@@ -4,7 +4,9 @@ Generate, Load scene, Export video and Export mesh (lib/core/ssdnerf_gui.py, dem
 Each scene becomes `<out-dir>/<scene>.avi`, a Motion-JPEG orbit of round(fps * sec) frames on the path of `video.surround_views`
 around the GUI's initial camera (pose `--camera-id` of DIR/pose, DIR/intrinsics.txt: any ShapeNet SRN scene directory or the
 reference's demo/camera_spiral_cars), rendered at `--res` rows by `BaseNeRF.render` on a white background with dt_gamma 0, as the GUI
-exports it.  Frames go from the renderer to the JPEG encoder on the device; only the compressed files reach the host.
+exports it.  Frames go from the renderer to the JPEG encoder on the device; only the compressed files reach the host.  With
+`--format mp4` each scene becomes `<out-dir>/<scene>.mp4` instead: all-intra H.264 at `--qp` (video.encode_h264, per --batch-frames
+batch), which browsers play as well.
 
   * --seed S: set_random_seed(S, deterministic=True), noise torch.randn((1,) + code_size) on the CPU, then val_uncond with
     `num_timesteps = --steps`; the scene is `seed_S`.  Seeds are sampled --batch-scenes at a time (each noise drawn after its own
@@ -41,12 +43,14 @@ def parse_args(argv=None):
     src.add_argument('--scene', nargs='+', help='saved scene files (.pth)')
     p.add_argument('--steps', type=int, default=20, help='diffusion sampling steps (num_timesteps)')
     p.add_argument('--batch-scenes', type=int, default=4, help='seeds sampled per batch')
-    p.add_argument('--out-dir', default='orbits', help='where <scene>.avi (and .stl / .pth) go')
+    p.add_argument('--out-dir', default='orbits', help='where <scene>.avi / .mp4 (and .stl / .pth) go')
     p.add_argument('--fps', type=int, default=30)
     p.add_argument('--sec', type=float, default=4.0, help='video length in seconds')
     p.add_argument('--res', type=int, default=256, help='video height in pixels (the width keeps the cameras\' aspect ratio)')
     p.add_argument('--batch-frames', type=int, default=30, help='frames rendered and encoded per batch')
-    p.add_argument('--quality', type=int, default=95, help='JPEG quality 1-100')
+    p.add_argument('--quality', type=int, default=95, help='JPEG quality 1-100 (avi)')
+    p.add_argument('--format', choices=('avi', 'mp4'), default='avi', help='Motion-JPEG AVI or H.264 MP4')
+    p.add_argument('--qp', type=int, default=20, help=f'H.264 quantiser {video.H264_MIN_QP}-51 (mp4; lower is larger and finer)')
     p.add_argument('--mesh', action='store_true', help='also write <scene>.stl')
     p.add_argument('--mesh-resolution', type=int, default=256)
     p.add_argument('--mesh-threshold', type=float, default=10)
@@ -59,6 +63,8 @@ def parse_args(argv=None):
             p.error(f'--{name.replace("_", "-")} must be >= 1')
     if not 1 <= args.quality <= 100:
         p.error('--quality must be in [1, 100]')
+    if not video.H264_MIN_QP <= args.qp <= 51:
+        p.error(f'--qp must be in [{video.H264_MIN_QP}, 51]')
     if not round(args.fps * args.sec) >= 1:
         p.error('--fps * --sec must give at least one frame')
     return args
@@ -151,13 +157,28 @@ def orbit_jpegs(model, code, bitfield, poses, intrinsics, hw, batch_frames, qual
     return files
 
 
+def orbit_h264(model, code, bitfield, poses, intrinsics, hw, batch_frames, qp, fps):
+    """(sps, pps, access units) of the orbit, rendered and encoded batch_frames at a time"""
+    samples, sps, pps = [], None, None
+    for lo in range(0, poses.size(0), batch_frames):
+        frames = render_frames(model, code, bitfield, poses[lo:lo + batch_frames], intrinsics, hw)
+        sps, pps, aus = video.encode_h264(frames, qp, fps, first_frame=lo)
+        samples += aus
+    return sps, pps, samples
+
+
 def export_scene(model, name, code, bitfield, geometry, args):
-    """writes <out_dir>/<name>.avi (and .stl / .pth); returns the written paths"""
+    """writes <out_dir>/<name>.avi or .mp4 (and .stl / .pth); returns the written paths"""
     poses, intrinsics, hw = geometry
     out = {}
-    jpegs = orbit_jpegs(model, code, bitfield, poses, intrinsics, hw, args.batch_frames, args.quality)
-    out['avi'] = os.path.join(args.out_dir, name + '.avi')
-    video.write_avi(out['avi'], jpegs, hw[1], hw[0], args.fps)
+    if args.format == 'mp4':
+        sps, pps, samples = orbit_h264(model, code, bitfield, poses, intrinsics, hw, args.batch_frames, args.qp, args.fps)
+        out['mp4'] = os.path.join(args.out_dir, name + '.mp4')
+        video.write_mp4(out['mp4'], sps, pps, samples, hw[1], hw[0], args.fps)
+    else:
+        jpegs = orbit_jpegs(model, code, bitfield, poses, intrinsics, hw, args.batch_frames, args.quality)
+        out['avi'] = os.path.join(args.out_dir, name + '.avi')
+        video.write_avi(out['avi'], jpegs, hw[1], hw[0], args.fps)
     if args.mesh:
         _, decoder = model._modules_for_eval()
         model.save_mesh(args.out_dir, decoder, code[None], [name], args.mesh_resolution, args.mesh_threshold)
@@ -169,7 +190,7 @@ def export_scene(model, name, code, bitfield, geometry, args):
 
 
 def main(argv=None):
-    """renders every scene; returns {scene name: {'avi': path, 'stl': path, 'pth': path}} in order"""
+    """renders every scene; returns {scene name: {'avi' or 'mp4': path, 'stl': path, 'pth': path}} in order"""
     args = parse_args(argv)
     cfg = Config.fromfile(args.config)
     if args.cfg_options is not None:

@@ -2,7 +2,9 @@
 lib/core/utils/camera_utils.py), without a window or ffmpeg.
 
 Frames are encoded on the device as baseline JPEG (csrc/jpeg.cu, byte-identical to cv2.imencode with libjpeg-turbo's defaults); only
-the compressed files are copied to the host, once per call, and written into a Motion-JPEG AVI that ffmpeg, VLC and mpv play."""
+the compressed files are copied to the host, once per call, and written into a Motion-JPEG AVI that ffmpeg, VLC and mpv play.
+Alternatively they are encoded as all-intra H.264 (csrc/h264.cu, oracle/h264_port.py) and written into an MP4 file that browsers
+also play."""
 import math
 import os
 import struct
@@ -17,6 +19,8 @@ from .datasets import load_intrinsics, load_pose
 AVI_MAX_BYTES = 1 << 30         # AVI 1.0 (no OpenDML): one RIFF list, kept under 1 GB for players that read 32-bit offsets signed
 AVIF_HASINDEX = 0x10
 AVIIF_KEYFRAME = 0x10
+MP4_MAX_BYTES = 1 << 32         # 32-bit stco chunk offsets and box sizes
+H264_MIN_QP = 10                # SSDNERF_H264_MIN_QP: below it Baseline's level codes cannot hold every 8-bit residual
 
 
 def encode_jpeg(frames, quality=95):
@@ -44,6 +48,104 @@ def encode_jpeg(frames, quality=95):
     off = offsets.cpu().tolist()
     data = out[:off[-1]].cpu().numpy().tobytes()
     return [data[off[i]:off[i + 1]] for i in range(n)]
+
+
+def encode_h264(frames, qp=20, fps=30, first_frame=0):
+    """(sps, pps, [access unit]) of CUDA RGB frames [n, h, w, 3], uint8 or float32 (float samples as in encode_jpeg): Constrained
+    Baseline H.264, every frame one IDR access unit of I_16x16 macroblocks at the constant `qp` (header section 13).  sps / pps are
+    NAL units without start code; each access unit is its slice NAL unit behind a 4-byte big-endian length (an MP4 sample).  `fps`
+    only selects the SPS's level; frame i's idr_pic_id is (first_frame + i) & 1, so the batches of one
+    video pass the index of their first frame.  Even h, w >= 2 within level 5.2 (36864 macroblocks, 543 per side); H264_MIN_QP <= qp <= 51."""
+    N.require_cuda(frames)
+    if frames.dim() != 4 or frames.shape[-1] != 3 or frames.dtype not in (torch.uint8, torch.float32):
+        raise ValueError(f'encode_h264: frames must be uint8 or float32 [n, h, w, 3], got {frames.dtype} {tuple(frames.shape)}')
+    if isinstance(qp, bool) or not isinstance(qp, (int, np.integer)) or not H264_MIN_QP <= int(qp) <= 51:
+        raise ValueError(f'encode_h264: qp must be an int in [{H264_MIN_QP}, 51], got {qp!r}')
+    fps = Fraction(fps).limit_denominator(1_000_000) if not isinstance(fps, Fraction) else fps
+    if fps <= 0 or fps.numerator >= 1 << 32 or fps.denominator >= 1 << 32:
+        raise ValueError(f'encode_h264: fps must be > 0, got {fps}')
+    n, h, w, _ = frames.shape
+    if n == 0:
+        raise ValueError('encode_h264: no frames')
+    L, dev, stream = N.lib(), frames.device, N.stream_ptr()
+    ws_bytes, out_bytes = L.ssdnerf_h264_workspace_bytes(n, h, w), L.ssdnerf_h264_output_bound(n, h, w)
+    if ws_bytes == 0:
+        raise ValueError(f'encode_h264: unsupported size h={h} w={w} (even sizes >= 2 up to level 5.2: 36864 macroblocks, 543 per side)')
+    frames = frames.contiguous()
+    work = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    out = torch.empty(out_bytes, dtype=torch.uint8, device=dev)
+    offsets = torch.empty(n + 3, dtype=torch.int64, device=dev)
+    fn = L.ssdnerf_h264_encode_u8 if frames.dtype == torch.uint8 else L.ssdnerf_h264_encode_f32
+    N.check(fn(N.ptr(frames), n, h, w, int(qp), fps.numerator, fps.denominator, int(first_frame) & 1, N.ptr(work), ws_bytes, N.ptr(out), out_bytes,
+               N.ptr(offsets), stream))
+    off = offsets.cpu().tolist()
+    data = out[:off[-1]].cpu().numpy().tobytes()
+    return data[off[0]:off[1]], data[off[1]:off[2]], [data[off[i]:off[i + 1]] for i in range(2, n + 2)]
+
+
+# ------------------------------------------------------------------------------------------------ MP4
+def _box(kind, *payload):
+    body = b''.join(payload)
+    return struct.pack('>I', 8 + len(body)) + kind + body
+
+
+def _full(kind, version, flags, *payload):
+    return _box(kind, struct.pack('>I', version << 24 | flags), *payload)
+
+
+def write_mp4(path, sps, pps, samples, width, height, fps):
+    """an MP4 file of one H.264 video track: `samples` are access units with 4-byte NAL lengths (encode_h264), width x height, at
+    `fps` frames per second (timescale and sample delta from Fraction(fps)).  Boxes: ftyp (isom, iso2, avc1, mp41), moov { mvhd,
+    trak { tkhd, mdia { mdhd, hdlr vide, minf { vmhd, dinf { dref url }, stbl { stsd { avc1 { avcC } }, stts, stsc, stsz, stco } } } } },
+    mdat; moov leads so a player can start before the whole file has arrived.  No stss: every sample is a sync sample.  Files over 4 GB
+    (32-bit stco offsets) are refused."""
+    samples = [bytes(s) for s in samples]
+    sps, pps, width, height = bytes(sps), bytes(pps), int(width), int(height)
+    if not samples:
+        raise ValueError('write_mp4: no frames')
+    if not (1 <= width <= 65535 and 1 <= height <= 65535):
+        raise ValueError(f'write_mp4: width and height must be in [1, 65535], got {width} x {height}')
+    if len(sps) < 4 or not pps:
+        raise ValueError('write_mp4: an SPS of at least 4 bytes and a PPS are needed')
+    fps = Fraction(fps).limit_denominator(1_000_000) if not isinstance(fps, Fraction) else fps
+    if fps <= 0:
+        raise ValueError(f'write_mp4: fps must be > 0, got {fps}')
+    n = len(samples)
+    timescale, delta = fps.numerator, fps.denominator
+    duration = n * delta
+    mdat_size = 8 + sum(len(s) for s in samples)
+    ident = struct.pack('>9i', 0x10000, 0, 0, 0, 0x10000, 0, 0, 0, 0x40000000)
+    avcc = _box(b'avcC', bytes([1, sps[1], sps[2], sps[3], 0xFF, 0xE1]), struct.pack('>H', len(sps)), sps, b'\x01',
+                struct.pack('>H', len(pps)), pps)
+    avc1 = _box(b'avc1', bytes(6), struct.pack('>H', 1), bytes(16), struct.pack('>HHIIIH', width, height, 0x480000, 0x480000, 0, 1),
+                bytes(32), struct.pack('>Hh', 0x18, -1), avcc)
+
+    def moov(mdat_start):
+        stbl = _box(b'stbl', _full(b'stsd', 0, 0, struct.pack('>I', 1), avc1),
+                    _full(b'stts', 0, 0, struct.pack('>III', 1, n, delta)),
+                    _full(b'stsc', 0, 0, struct.pack('>IIII', 1, 1, n, 1)),
+                    _full(b'stsz', 0, 0, struct.pack('>II', 0, n), b''.join(struct.pack('>I', len(s)) for s in samples)),
+                    _full(b'stco', 0, 0, struct.pack('>II', 1, mdat_start + 8)))
+        minf = _box(b'minf', _full(b'vmhd', 0, 1, bytes(8)),
+                    _box(b'dinf', _full(b'dref', 0, 0, struct.pack('>I', 1), _full(b'url ', 0, 1))), stbl)
+        mdia = _box(b'mdia', _full(b'mdhd', 0, 0, struct.pack('>IIIIHH', 0, 0, timescale, duration, 0x55C4, 0)),
+                    _full(b'hdlr', 0, 0, bytes(4), b'vide', bytes(12), b'VideoHandler\0'), minf)
+        tkhd = _full(b'tkhd', 0, 3, struct.pack('>IIIII', 0, 0, 1, 0, duration), bytes(8), struct.pack('>hhhH', 0, 0, 0, 0), ident,
+                     struct.pack('>II', width << 16, height << 16))
+        mvhd = _full(b'mvhd', 0, 0, struct.pack('>IIIIIH', 0, 0, timescale, duration, 0x10000, 0x100), bytes(10), ident, bytes(24),
+                     struct.pack('>I', 2))
+        return _box(b'moov', mvhd, _box(b'trak', tkhd, mdia))
+    ftyp = _box(b'ftyp', b'isom', struct.pack('>I', 0x200), b'isomiso2avc1mp41')
+    head = len(ftyp) + len(moov(0))
+    total = head + mdat_size
+    if total > MP4_MAX_BYTES - 1 or duration >= 1 << 32:
+        raise ValueError(f'write_mp4: {total} bytes exceed the 4 GB limit of 32-bit MP4 offsets (stco); write fewer or smaller '
+                         'frames per file')
+    os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
+    with open(path, 'wb') as f:
+        f.write(ftyp + moov(head) + struct.pack('>I', mdat_size) + b'mdat')
+        for s in samples:
+            f.write(s)
 
 
 # ------------------------------------------------------------------------------------------------ Motion-JPEG AVI
